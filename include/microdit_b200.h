@@ -280,6 +280,22 @@ MD_API int md_edm_output(const float* ftok, const int32_t* ids_restore, const fl
                          const float* coef, float* fx, float* dx, int64_t B, int64_t C, int64_t H, int64_t W,
                          int64_t p, int64_t Tk, void* stream);
 
+/* ----------------------------------------------- adjoints for the differentiable DiT.forward (VJP) */
+/* adjoint of the unmask_tokens + unpatchify of md_edm_output for the raw output F (utils.py:417-426,
+ * dit.py:566-575): dF f32 [B,C,H,W] -> dftok [B*Tk, p*p*C] (column (i*p+j)*C+c; bf16, f32 with prec=1) for the kept
+ * tokens only: keep_rows int32 [B*Tk] (md_mask_sort's keep_rows) or NULL (Tk = T).  Masked tokens output the
+ * non-trainable mask_token buffer (dit.py:440-443) and receive no gradient. */
+MD_API int md_unpatchify_bwd(const float* dF, const int32_t* keep_rows, void* dftok, int64_t B, int64_t C, int64_t H,
+                             int64_t W, int64_t p, int64_t Tk, int prec, void* stream);
+/* adjoint of md_patchify (col2im of the patch-embed conv, dit.py:479; column (c*p+i)*p+j): dpatches f32 [B*T, C*p*p],
+ * scale f32 [B] or NULL -> dx f32 [B,C,H,W] (written, not accumulated).  Inputs are f32 in both precisions. */
+MD_API int md_patchify_bwd(const float* dpatches, const float* scale, float* dx, int64_t B, int64_t C, int64_t H,
+                           int64_t W, int64_t p, int prec, void* stream);
+/* adjoint of md_timestep_embed (utils.py:265-281): dt[b] = sum_i dfreq[b,i] * d[cos|sin](t[b]*w_i)/dt; dfreq f32
+ * [B, dim], t f32 [B], dt f32 [B] (written).  One block per sample with a fixed reduction order: deterministic. */
+MD_API int md_timestep_embed_bwd(const float* dfreq, const float* t, float* dt, int64_t B, int64_t dim, int prec,
+                                 void* stream);
+
 /* ------------------------------------------------------------------------------------ utilities */
 /* mean over the L tokens of each sample (dit.py:484): x f32 [B,L,D] -> bf16 [B,D]; bwd: dx[b,l,:] += d[b,:]/L */
 MD_API int md_mean_tokens_fwd(const float* x, void* out, int64_t B, int64_t L, int64_t D, int prec, void* stream);

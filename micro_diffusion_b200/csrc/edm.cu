@@ -142,6 +142,69 @@ __global__ void edm_output_kernel(const float* __restrict__ ftok, const int32_t*
   }
 }
 
+// ------------------------------------------------------------------------------------- adjoints (DiT VJP)
+// Adjoint of the un-mask + unpatchify of edm_output_kernel for the raw output F: one thread per element of dftok
+// [B*Tk, p*p*C] (column (i*p+j)*C+c, coalesced writes).  Masked tokens show the non-trainable mask_token buffer, so only
+// the kept tokens have a gradient.
+template <typename AT>
+__global__ void unpatchify_bwd_kernel(const float* __restrict__ dF, const int32_t* __restrict__ keep_rows,
+                                      AT* __restrict__ dftok, int B, int C, int H, int W, int p, int Tk) {
+  const int gw = W / p, T = gw * (H / p), Nf = p * p * C;
+  const long long total = 1LL * B * Tk * Nf;
+  for (long long i = 1LL * blockIdx.x * blockDim.x + threadIdx.x; i < total; i += 1LL * gridDim.x * blockDim.x) {
+    const int col = static_cast<int>(i % Nf);
+    const long long row = i / Nf;  // b * Tk + j
+    const int b = static_cast<int>(row / Tk);
+    const int tok = keep_rows ? keep_rows[row] % T : static_cast<int>(row % Tk);  // keep_rows holds b*T + token
+    const int c = col % C, q = col / C;
+    const long long src = ((1LL * b * C + c) * H + (tok / gw) * p + q / p) * W + (tok % gw) * p + q % p;
+    st1a(dftok + i, dF[src]);
+  }
+}
+
+// Adjoint of patchify_kernel (col2im of the stride-p patch-embed conv, column (c*p+i)*p+j): the patches do not overlap,
+// so every pixel reads exactly one element.  One thread per pixel of dx (coalesced writes).
+__global__ void patchify_bwd_kernel(const float* __restrict__ dpatches, const float* __restrict__ scale,
+                                    float* __restrict__ dx, int B, int C, int H, int W, int p) {
+  const int gw = W / p, gh = H / p, Kp = C * p * p;
+  const long long total = 1LL * B * C * H * W;
+  for (long long i = 1LL * blockIdx.x * blockDim.x + threadIdx.x; i < total; i += 1LL * gridDim.x * blockDim.x) {
+    const int x = static_cast<int>(i % W);
+    long long r = i / W;
+    const int y = static_cast<int>(r % H); r /= H;
+    const int c = static_cast<int>(r % C);
+    const int b = static_cast<int>(r / C);
+    const long long tok = 1LL * b * gh * gw + 1LL * (y / p) * gw + x / p;
+    const float v = dpatches[tok * Kp + (c * p + y % p) * p + x % p];
+    dx[i] = scale ? scale[b] * v : v;
+  }
+}
+
+// Adjoint of timestep_embed_kernel: dt[b] = sum_i f_i * (dfreq[b, half+i] cos(t f_i) - dfreq[b, i] sin(t f_i)).  One
+// block per sample; every thread sums a fixed stride of frequencies, then a fixed-order warp / block reduction, so the
+// result does not depend on scheduling (no atomics).
+__global__ void __launch_bounds__(256)
+timestep_embed_bwd_kernel(const float* __restrict__ dfreq, const float* __restrict__ t, float* __restrict__ dt, int dim) {
+  const long long b = blockIdx.x;
+  const int half = dim / 2;
+  const float tv = t[b];
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < half; i += blockDim.x) {
+    const float freq = expf(-9.210340371976184f * static_cast<float>(i) / static_cast<float>(half));
+    const float a = tv * freq;
+    acc += freq * (dfreq[b * dim + half + i] * cosf(a) - dfreq[b * dim + i] * sinf(a));
+  }
+  acc = warp_sum(acc);
+  __shared__ float part[8];
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < (blockDim.x >> 5); ++w) s += part[w];
+    dt[b] = s;
+  }
+}
+
 // ------------------------------------------------------------------------------------- mask_sort
 // One block per sample: bitonic sort of (noise, index) ascending in shared memory (n = next pow2 >= T).
 __global__ void __launch_bounds__(1024)
@@ -273,6 +336,42 @@ extern "C" int md_edm_output(const float* ftok, const int32_t* ids_restore, cons
                                                                           dx, (int)B, (int)C, (int)H, (int)W, (int)p,
                                                                           (int)Tk);
   return check_launch("md_edm_output");
+}
+
+extern "C" int md_unpatchify_bwd(const float* dF, const int32_t* keep_rows, void* dftok, int64_t B, int64_t C, int64_t H,
+                                 int64_t W, int64_t p, int64_t Tk, int prec, void* stream) {
+  if (B == 0) return 0;
+  if (!dF || !dftok) return md_set_error(MD_ERR_INVALID, "md_unpatchify_bwd: null pointer");
+  if (p <= 0 || H % p != 0 || W % p != 0)
+    return md_set_error(MD_ERR_INVALID, "md_unpatchify_bwd: H, W must be multiples of p");
+  if (Tk < 1 || Tk > (H / p) * (W / p) || (!keep_rows && Tk != (H / p) * (W / p)))
+    return md_set_error(MD_ERR_INVALID, "md_unpatchify_bwd: Tk must be in [1, T] (T without keep_rows)");
+  if (prec != 0 && prec != 1) return md_set_error(MD_ERR_INVALID, "md_unpatchify_bwd: prec must be 0 or 1");
+  MD_WITH_ACT(prec, unpatchify_bwd_kernel<AT><<<grid_for(B * Tk * C * p * p, 256), 256, 0, ST(stream)>>>(
+                        dF, keep_rows, AP(AT, dftok), (int)B, (int)C, (int)H, (int)W, (int)p, (int)Tk));
+  return check_launch("md_unpatchify_bwd");
+}
+
+extern "C" int md_patchify_bwd(const float* dpatches, const float* scale, float* dx, int64_t B, int64_t C, int64_t H,
+                               int64_t W, int64_t p, int prec, void* stream) {
+  if (B == 0) return 0;
+  if (!dpatches || !dx) return md_set_error(MD_ERR_INVALID, "md_patchify_bwd: null pointer");
+  if (p <= 0 || H % p != 0 || W % p != 0)
+    return md_set_error(MD_ERR_INVALID, "md_patchify_bwd: H, W must be multiples of p");
+  if (prec != 0 && prec != 1) return md_set_error(MD_ERR_INVALID, "md_patchify_bwd: prec must be 0 or 1");
+  patchify_bwd_kernel<<<grid_for(B * C * H * W, 256), 256, 0, ST(stream)>>>(dpatches, scale, dx, (int)B, (int)C, (int)H,
+                                                                           (int)W, (int)p);
+  return check_launch("md_patchify_bwd");
+}
+
+extern "C" int md_timestep_embed_bwd(const float* dfreq, const float* t, float* dt, int64_t B, int64_t dim, int prec,
+                                     void* stream) {
+  if (B == 0) return 0;
+  if (!dfreq || !t || !dt) return md_set_error(MD_ERR_INVALID, "md_timestep_embed_bwd: null pointer");
+  if (dim < 2) return md_set_error(MD_ERR_INVALID, "md_timestep_embed_bwd: dim must be >= 2");
+  if (prec != 0 && prec != 1) return md_set_error(MD_ERR_INVALID, "md_timestep_embed_bwd: prec must be 0 or 1");
+  timestep_embed_bwd_kernel<<<(unsigned)B, 256, 0, ST(stream)>>>(dfreq, t, dt, (int)dim);
+  return check_launch("md_timestep_embed_bwd");
 }
 
 extern "C" int md_mask_sort(const float* noise, int32_t* ids_shuffle, int32_t* ids_restore, float* mask,

@@ -37,15 +37,43 @@ class Engine:
         self.L = None  # caption length, set per call
 
     # ================================================================== helpers
+    # True while backward_output(param_grads=False) runs: every weight-gradient GEMM, bias column sum and LayerNorm
+    # d gamma is skipped and the flat gradient buffer is not touched
+    _skip_wgrad = False
+
+    def _gv(self, name):
+        """Gradient view of one parameter, or None while weight gradients are skipped."""
+        return None if self._skip_wgrad else self.store.g[name]
+
+    def _Gv(self, name):
+        """Gradient view of a GEMM group (ParamStore.G), or None while weight gradients are skipped."""
+        return None if self._skip_wgrad else self.store.G(name)
+
+    def _colsum(self, x, out):
+        """Bias gradient out += column sums of x (skipped when out is None)."""
+        if out is not None:
+            self.ops.colsum(x, out)
+
     def _wgrad(self, dY, X, G):
         """G[P,Q] (+)= dY[r,P]^T X[r,Q]  (reduction over the rows r); the library picks the split of the
-        reduction that fills the SMs (splits=0)."""
-        self.ops.gemm(dY, X, G, layout=TN, epi=EPI_ATOMIC, splits=0)
+        reduction that fills the SMs (splits=0).  Skipped when G is None."""
+        if G is not None:
+            self.ops.gemm(dY, X, G, layout=TN, epi=EPI_ATOMIC, splits=0)
 
     def _wgrad_w12(self, name, dU, X):
         """Weight gradient of a w1 | w2 stack; with the fused SwiGLU layout the rows of d u arrive interleaved."""
-        self.ops.gemm(dU, X, self.store.G(name), layout=TN, epi=EPI_ATOMIC, splits=0,
-                      row_interleave=self.store.interleave.get(name, 0))
+        if not self._skip_wgrad:
+            self.ops.gemm(dU, X, self.store.G(name), layout=TN, epi=EPI_ATOMIC, splits=0,
+                          row_interleave=self.store.interleave.get(name, 0))
+
+    def _transposed(self, name):
+        """Transposed bf16 copy of a matrix the training step never needs one of (the patch embed and the first caption
+        projection, whose inputs are data): made on demand for the input gradients of backward_output."""
+        st = self.store
+        g = st.layout.groups[name]
+        wt = self.ops.empty((g.cols, g.rows), BF16)
+        self.ops.cast_transpose(st.flat[g.offset: g.offset + g.numel].view(g.rows, g.cols), None, wt)
+        return wt
 
     def _swiglu_fwd(self, name_w12, x, u, hact):
         """u = x W12^T, hact = silu(u1) * u2 (dit.py:88-89): one GEMM when the stack is interleaved, GEMM + pass otherwise."""
@@ -82,7 +110,7 @@ class Engine:
     def _kv_bwd(self, group, dkv_all, ykv, dykv):
         """Weight gradient of the stacked kv_linear and the gradient flowing into the caption tokens."""
         o, st = self.ops, self.store
-        self._wgrad(dkv_all, ykv, st.G(group))
+        self._wgrad(dkv_all, ykv, self._Gv(group))
         o.gemm(dkv_all, st.WT(group), dykv, epi=EPI_RESID, res=dykv)
 
     # ================================================================== block forward
@@ -188,7 +216,7 @@ class Engine:
         _ffn_gate_args of the block the chain enters next -- this block's last LayerNorm backward then emits that
         block's dy_in, which is returned."""
         o, st, cfg = self.ops, self.store, self.cfg
-        P, G = st.p, st.g
+        P = st.p
         n, D, h, f, hd = bs.name, bs.dim, bs.attn_dim, bs.ffn_dim, cfg.head_dim
         M = B * T
         fuse = self.fuse_ln
@@ -204,7 +232,7 @@ class Engine:
         if not bs.moe:
             du = o.empty((M, 2 * f), BF16)
             self._swiglu_bwd(n + ".mlp.w12", n + ".mlp.w3.weight", dy, sv.u, du)
-            self._wgrad(dy, sv.hact, st.G(n + ".mlp.w3.weight"))
+            self._wgrad(dy, sv.hact, self._Gv(n + ".mlp.w3.weight"))
             o.gemm(du, st.WT(n + ".mlp.w12"), dxm)
             self._wgrad_w12(n + ".mlp.w12", du, sv.xm3)
         else:
@@ -218,22 +246,23 @@ class Engine:
                 dhact = o.empty((E, B * k, f), BF16)
                 o.gemm(dh2, st.W(n + ".mlp.w2"), dhact)
                 o.act_bwd(dhact, sv.hpre, dhpre, ACT_ERF)
-            self._wgrad(sv.hact, dh2, st.G(n + ".mlp.w2"))
+            self._wgrad(sv.hact, dh2, self._Gv(n + ".mlp.w2"))
             dxin = o.empty((E, B * k, D), BF16)
             o.gemm(dhpre, st.W(n + ".mlp.w1"), dxin)
-            self._wgrad(sv.xin, dhpre, st.G(n + ".mlp.w1"))
+            self._wgrad(sv.xin, dhpre, self._Gv(n + ".mlp.w1"))
             dscores = o.empty((M, E), F32)
             o.moe_dx_bwd(dxin, sv.inv, dgval, sv.probs, P[n + ".mlp.gate.weight"], dscores, dxm, B, T, E, k)
-            o.moe_gate_wgrad(dscores, sv.xm3, G[n + ".mlp.gate.weight"])
+            if not self._skip_wgrad:
+                o.moe_gate_wgrad(dscores, sv.xm3, self._gv(n + ".mlp.gate.weight"))
         dy = o.empty((M, D), BF16)
         o.ln_bwd(dxm, sv.x2, sv.mean3, sv.rstd3, gamma=P[n + ".norm3.weight"], scale=sc_m, T=T, dx=dx, dx_mode=0,
-                 dgamma=G[n + ".norm3.weight"], dshift=dsh_m, dscale=dsc_m, dy_next=dy if fuse else None)
+                 dgamma=self._gv(n + ".norm3.weight"), dshift=dsh_m, dscale=dsc_m, dy_next=dy if fuse else None)
         # ---- cross attention branch (no gate, no modulation): dy = bf16(dx)
         if not fuse:
             o.gate_bwd(dx, dy, T=T)
         datt2 = o.empty((M, D), BF16)
         o.gemm(dy, st.WT(n + ".cross_attn.proj.weight"), datt2)
-        self._wgrad(dy, sv.att2, st.G(n + ".cross_attn.proj.weight"))
+        self._wgrad(dy, sv.att2, self._Gv(n + ".cross_attn.proj.weight"))
         dqx = o.empty((M, D), BF16)
         delta = o.empty((B, bs.xheads, T), F32)
         o.attn_bwd(datt2, sv.qx, sv.kv[:, :D], sv.kv[:, D:], sv.att2, sv.lse2, delta, dqx, dkv[:, :D], dkv[:, D:], B,
@@ -242,19 +271,19 @@ class Engine:
         o.rownorm_bwd(dkv[:, :D], sv.kv[:, :D], sv.rk2)
         dxn2 = o.empty((M, D), BF16)
         o.gemm(dqx, st.WT(n + ".cross_attn.q_linear.weight"), dxn2)
-        self._wgrad(dqx, sv.xn2, st.G(n + ".cross_attn.q_linear.weight"))
+        self._wgrad(dqx, sv.xn2, self._Gv(n + ".cross_attn.q_linear.weight"))
         dy = o.empty((M, D), BF16)
         if fuse:
             o.ln_bwd(dxn2, sv.x1, sv.mean2, sv.rstd2, gamma=P[n + ".norm2.weight"], T=T, dx=dx, dx_mode=0,
-                     dgamma=G[n + ".norm2.weight"], dy_next=dy, y_next=sv.ya, gate_next=g_a, dgate_next=dg_a)
+                     dgamma=self._gv(n + ".norm2.weight"), dy_next=dy, y_next=sv.ya, gate_next=g_a, dgate_next=dg_a)
         else:
             o.ln_bwd(dxn2, sv.x1, sv.mean2, sv.rstd2, gamma=P[n + ".norm2.weight"], T=T, dx=dx, dx_mode=0,
-                     dgamma=G[n + ".norm2.weight"])
+                     dgamma=self._gv(n + ".norm2.weight"))
             o.gate_bwd(dx, dy, y=sv.ya, gate=g_a, dgate=dg_a, T=T)
         # ---- self attention branch
         datt = o.empty((M, h), BF16)
         o.gemm(dy, st.WT(n + ".attn.proj.weight"), datt)
-        self._wgrad(dy, sv.att, st.G(n + ".attn.proj.weight"))
+        self._wgrad(dy, sv.att, self._Gv(n + ".attn.proj.weight"))
         dqkv = o.empty((M, 3 * h), BF16)
         delta = o.empty((B, bs.heads, T), F32)
         o.attn_bwd(datt, sv.qkv[:, :h], sv.qkv[:, h:2 * h], sv.qkv[:, 2 * h:], sv.att, sv.lse, delta, dqkv[:, :h],
@@ -262,10 +291,10 @@ class Engine:
         o.rownorm_bwd(dqkv[:, :2 * h], sv.qkv[:, :2 * h], sv.rqk, nslice=2)
         dxm1 = o.empty((M, D), BF16)
         o.gemm(dqkv, st.WT(n + ".attn.qkv.weight"), dxm1)
-        self._wgrad(dqkv, sv.xm, st.G(n + ".attn.qkv.weight"))
+        self._wgrad(dqkv, sv.xm, self._Gv(n + ".attn.qkv.weight"))
         dy_out = o.empty((M, D), BF16) if (fuse and nxt is not None) else None
         o.ln_bwd(dxm1, sv.x, sv.mean1, sv.rstd1, gamma=P[n + ".norm1.weight"], scale=sc_a, T=T, dx=dx, dx_mode=0,
-                 dgamma=G[n + ".norm1.weight"], dshift=dsh_a, dscale=dsc_a, dy_next=dy_out,
+                 dgamma=self._gv(n + ".norm1.weight"), dshift=dsh_a, dscale=dsc_a, dy_next=dy_out,
                  **(nxt if dy_out is not None else {}))
         return dy_out
 
@@ -350,18 +379,21 @@ class Engine:
         o.gemm(s.cact, st.W("ada"), s.mod, epi=EPI_F32, bias=st.ada_bias)
         return s
 
-    def _stem_bwd(self, s, dmod, dy2, B):
-        """dmod f32 [B, ada_rows] (filled by the blocks), dy2 f32 [B*L, D] grad wrt the caption tokens."""
+    def _stem_bwd(self, s, dmod, dy2, B, want_dt=True, want_dy=True):
+        """dmod f32 [B, ada_rows] (filled by the blocks), dy2 f32 [B*L, D] grad wrt the caption tokens.  Returns the bf16
+        gradients at the pre-activations of t_embedder.mlp.0 and y_embedder.y_proj.fc1 (the input-gradient exits of
+        backward_output).  While weight gradients are skipped, the timestep branch runs only for want_dt and the caption
+        branch only for want_dy."""
         o, st, cfg = self.ops, self.store, self.cfg
-        P, G = st.p, st.g
+        P = st.p
         D, hd, L = cfg.dim, cfg.head_dim, s.L
         R = B * L
         H = D // hd
         # ---- adaLN stack
         dmod_bf = o.empty(tuple(dmod.shape), BF16)
         o.cast_bf16(dmod, dmod_bf)
-        self._wgrad(dmod_bf, s.cact, st.G("ada"))
-        o.colsum(dmod, st.g_ada_bias)
+        self._wgrad(dmod_bf, s.cact, self._Gv("ada"))
+        self._colsum(dmod, None if self._skip_wgrad else st.g_ada_bias)
         dcact = o.zeros((B, D), F32)  # K = sum(6D) ~ 2e5 with only a handful of output tiles: split the reduction
         o.gemm(dmod_bf, st.WT("ada"), dcact, epi=EPI_ATOMIC, splits=0)
         dc = o.empty((B, D), F32)
@@ -369,26 +401,30 @@ class Engine:
         dc_bf = o.empty((B, D), BF16)
         o.cast_bf16(dc, dc_bf)
         # ---- timestep embedder (c = temb + pooled: dc flows to both)
-        o.colsum(dc, G["t_embedder.mlp.2.bias"])
-        self._wgrad(dc_bf, s.t1, st.G("t_embedder.mlp.2.weight"))
-        dt1 = o.empty((B, D), BF16)
-        o.gemm(dc_bf, st.WT("t_embedder.mlp.2.weight"), dt1)
-        dt1pre = o.empty((B, D), BF16)
-        o.act_bwd(dt1, s.t1pre, dt1pre, ACT_TANH)
-        o.colsum(dt1pre, G["t_embedder.mlp.0.bias"])
-        self._wgrad(dt1pre, s.tfreq, st.G("t_embedder.mlp.0.weight"))
+        self._colsum(dc, self._gv("t_embedder.mlp.2.bias"))
+        self._wgrad(dc_bf, s.t1, self._Gv("t_embedder.mlp.2.weight"))
+        dt1pre = None
+        if want_dt or not self._skip_wgrad:
+            dt1 = o.empty((B, D), BF16)
+            o.gemm(dc_bf, st.WT("t_embedder.mlp.2.weight"), dt1)
+            dt1pre = o.empty((B, D), BF16)
+            o.act_bwd(dt1, s.t1pre, dt1pre, ACT_TANH)
+            self._colsum(dt1pre, self._gv("t_embedder.mlp.0.bias"))
+            self._wgrad(dt1pre, s.tfreq, self._Gv("t_embedder.mlp.0.weight"))
+        if not (want_dy or not self._skip_wgrad):
+            return dt1pre, None
         # ---- pooled caption Mlp
-        o.colsum(dc, G["pooled_y_emb_process.fc2.bias"])
-        self._wgrad(dc_bf, s.p1n, st.G("pooled_y_emb_process.fc2.weight"))
+        self._colsum(dc, self._gv("pooled_y_emb_process.fc2.bias"))
+        self._wgrad(dc_bf, s.p1n, self._Gv("pooled_y_emb_process.fc2.weight"))
         dp1n = o.empty((B, D), BF16)
         o.gemm(dc_bf, st.WT("pooled_y_emb_process.fc2.weight"), dp1n)
         dp1 = o.empty((B, D), BF16)
         o.ln_bwd(dp1n, s.p1, s.m_p, s.r_p, gamma=P["pooled_y_emb_process.norm.weight"], T=1, dx=dp1, dx_mode=1,
-                 dgamma=G["pooled_y_emb_process.norm.weight"])
+                 dgamma=self._gv("pooled_y_emb_process.norm.weight"))
         dp1pre = o.empty((B, D), BF16)
         o.act_bwd(dp1, s.p1pre, dp1pre, ACT_TANH)
-        o.colsum(dp1pre, G["pooled_y_emb_process.fc1.bias"])
-        self._wgrad(dp1pre, s.pool, st.G("pooled_y_emb_process.fc1.weight"))
+        self._colsum(dp1pre, self._gv("pooled_y_emb_process.fc1.bias"))
+        self._wgrad(dp1pre, s.pool, self._Gv("pooled_y_emb_process.fc1.weight"))
         dpool = o.empty((B, D), F32)
         o.gemm(dp1pre, st.WT("pooled_y_emb_process.fc1.weight"), dpool, epi=EPI_F32)
         o.mean_tokens_bwd(dpool, dy2, B, L)
@@ -398,38 +434,39 @@ class Engine:
         o.gate_bwd(dy2, dyb, T=L)
         du = o.empty((R, 2 * fp), BF16)
         self._swiglu_bwd("y_emb_preprocess.mlp.w12", "y_emb_preprocess.mlp.w3.weight", dyb, s.u, du)
-        self._wgrad(dyb, s.hact, st.G("y_emb_preprocess.mlp.w3.weight"))
+        self._wgrad(dyb, s.hact, self._Gv("y_emb_preprocess.mlp.w3.weight"))
         dyn = o.empty((R, D), BF16)
         o.gemm(du, st.WT("y_emb_preprocess.mlp.w12"), dyn)
         self._wgrad_w12("y_emb_preprocess.mlp.w12", du, s.yn2)
         o.ln_bwd(dyn, s.y1, s.m2, s.r2, gamma=P["y_emb_preprocess.norm2.weight"], T=L, dx=dy2, dx_mode=0,
-                 dgamma=G["y_emb_preprocess.norm2.weight"])
+                 dgamma=self._gv("y_emb_preprocess.norm2.weight"))
         # ---- prompt block: self attention
         o.gate_bwd(dy2, dyb, T=L)
         datt = o.empty((R, D), BF16)
         o.gemm(dyb, st.WT("y_emb_preprocess.attn.proj.weight"), datt)
-        self._wgrad(dyb, s.att, st.G("y_emb_preprocess.attn.proj.weight"))
+        self._wgrad(dyb, s.att, self._Gv("y_emb_preprocess.attn.proj.weight"))
         dqkv = o.empty((R, 3 * D), BF16); delta = o.empty((B, H, L), F32)
         o.attn_bwd(datt, s.qkv[:, :D], s.qkv[:, D:2 * D], s.qkv[:, 2 * D:], s.att, s.lse, delta, dqkv[:, :D],
                    dqkv[:, D:2 * D], dqkv[:, 2 * D:], B, H, L, L, hd)
         o.rownorm_bwd(dqkv[:, :2 * D], s.qkv[:, :2 * D], s.rqk, nslice=2)
         o.gemm(dqkv, st.WT("y_emb_preprocess.attn.qkv.weight"), dyn)
-        self._wgrad(dqkv, s.yn1, st.G("y_emb_preprocess.attn.qkv.weight"))
+        self._wgrad(dqkv, s.yn1, self._Gv("y_emb_preprocess.attn.qkv.weight"))
         o.ln_bwd(dyn, s.y0, s.m1, s.r1, gamma=P["y_emb_preprocess.norm1.weight"], T=L, dx=dy2, dx_mode=0,
-                 dgamma=G["y_emb_preprocess.norm1.weight"])
+                 dgamma=self._gv("y_emb_preprocess.norm1.weight"))
         # ---- caption projection
         o.gate_bwd(dy2, dyb, T=L)
-        o.colsum(dy2, G["y_embedder.y_proj.fc2.bias"])
-        self._wgrad(dyb, s.a1n, st.G("y_embedder.y_proj.fc2.weight"))
+        self._colsum(dy2, self._gv("y_embedder.y_proj.fc2.bias"))
+        self._wgrad(dyb, s.a1n, self._Gv("y_embedder.y_proj.fc2.weight"))
         da1n = o.empty((R, D), BF16)
         o.gemm(dyb, st.WT("y_embedder.y_proj.fc2.weight"), da1n)
         da1 = o.empty((R, D), BF16)
         o.ln_bwd(da1n, s.a1, s.m_a, s.r_a, gamma=P["y_embedder.y_proj.norm.weight"], T=L, dx=da1, dx_mode=1,
-                 dgamma=G["y_embedder.y_proj.norm.weight"])
+                 dgamma=self._gv("y_embedder.y_proj.norm.weight"))
         da1pre = o.empty((R, D), BF16)
         o.act_bwd(da1, s.a1pre, da1pre, ACT_TANH)
-        o.colsum(da1pre, G["y_embedder.y_proj.fc1.bias"])
-        self._wgrad(da1pre, s.ycap, st.G("y_embedder.y_proj.fc1.weight"))
+        self._colsum(da1pre, self._gv("y_embedder.y_proj.fc1.bias"))
+        self._wgrad(da1pre, s.ycap, self._Gv("y_embedder.y_proj.fc1.weight"))
+        return dt1pre, da1pre
 
     # ================================================================== denoiser forward
     def prompt_cache(self, cap):
@@ -474,7 +511,7 @@ class Engine:
         p, D, Dm = cfg.patch_size, cfg.dim, cfg.mixer_dim
         T = (Hh // p) * (Ww // p)
         assert T == cfg.num_patches and C == cfg.in_channels, "input does not match the model's latent shape"
-        c = NS(B=B, T=T, mask_ratio=mask_ratio, lat=lat)
+        c = NS(B=B, T=T, mask_ratio=mask_ratio, lat=lat, raw_t=raw_t)
         # ---- noise + preconditioning + im2col (model.py:182-188, 153-166)
         c.patches = o.empty((B * T, cfg.patch_dim), BF16)
         if raw_t is None:
@@ -591,31 +628,80 @@ class Engine:
         o.edm_output(c.ftok, c.ids_restore, self.mask_token.reshape(-1), c.xn, c.coef, fx, dx, self.cfg.patch_size, c.Tk)
         return dx, fx, c.mask
 
-    def forward_raw(self, x, t, cap, mask_ratio=0.0, mask_noise=None):
-        """DiT.forward_without_cfg (dit.py:455-519) without gradients: {'sample': F_x, 'mask': mask}."""
+    def forward_raw(self, x, t, cap, mask_ratio=0.0, mask_noise=None, keep=False):
+        """DiT.forward_without_cfg (dit.py:455-519): (F_x, mask).  keep=True saves the activations and returns
+        (F_x, mask, ctx) for backward_output(ctx, ...)."""
         o = self.ops
-        c = self._denoiser_fwd(x, None, None, None, cap, None, mask_ratio, mask_noise, None, keep=False, raw_t=t)
+        c = self._denoiser_fwd(x, None, None, None, cap, None, mask_ratio, mask_noise, None, keep=keep, raw_t=t)
         B, C, Hh, Ww = x.shape
         fx = o.empty((B, C, Hh, Ww), F32)
         o.edm_output(c.ftok, c.ids_restore, self.mask_token.reshape(-1), None, None, fx, None, self.cfg.patch_size, c.Tk)
-        return fx, c.mask
+        return (fx, c.mask, c) if keep else (fx, c.mask)
 
     def backward(self, c, gscale):
         """Accumulate d(loss * gscale) / d(parameters) into the flat gradient buffer."""
+        o, cfg = self.ops, self.cfg
+        dmod, dy2 = self._bwd_accumulators(c)
+        # ---- loss -> final layer
+        dftok = o.empty((c.B * c.Tk, cfg.patch_dim), BF16)
+        o.edm_loss_bwd(c.ftok, c.keep_rows, c.lat, c.xn, c.coef, gscale, dftok, cfg.patch_size, c.Tk)
+        self._backward_from_tokens(c, dftok, dmod, dy2)
+
+    def backward_output(self, c, dF, *, param_grads: bool, want_dx: bool, want_dt: bool, want_dy: bool):
+        """Vector-Jacobian product of forward_raw(..., keep=True) for the cotangent dF (f32 [B,C,H,W]) of F_x.
+
+        param_grads=True accumulates d<F_x, dF>/d(parameters) into the flat gradient buffer like backward();
+        param_grads=False (every DiT parameter frozen) skips all weight gradients and writes nothing there.
+        Returns (dx f32 [B,C,H,W], dt f32 [B], dy f32 [B*L, caption_channels]), None where not wanted: the
+        gradients wrt forward_raw's x, t and (the bf16 storage of) the caption."""
         o, st, cfg = self.ops, self.store, self.cfg
-        P, G = st.p, st.g
+        B, T, Tk, p = c.B, c.T, c.Tk, cfg.patch_size
+        dmod, dy2 = self._bwd_accumulators(c)
+        dftok = o.empty((B * Tk, cfg.patch_dim), BF16)
+        o.unpatchify_bwd(dF, c.keep_rows, dftok, p, Tk)
+        self._skip_wgrad = not param_grads
+        try:
+            dx0b, dt1pre, da1pre = self._backward_from_tokens(c, dftok, dmod, dy2, grads_ready_hook=False,
+                                                              want_dx0=want_dx, want_dt=want_dt, want_dy=want_dy)
+        finally:
+            self._skip_wgrad = False
+        dx = dt = dy = None
+        if want_dx:  # patch-embed dgrad (N = C*p*p) + col2im
+            dpatches = o.empty((B * T, cfg.patch_dim), F32)
+            o.gemm(dx0b, self._transposed("x_embedder.proj.weight"), dpatches, epi=EPI_F32)
+            dx = o.empty(tuple(c.lat.shape), F32)
+            o.patchify_bwd(dpatches, None, dx, p)
+        if want_dt:  # t_embedder.mlp.0 dgrad + the sinusoid's adjoint
+            dfreq = o.empty((B, cfg.freq_dim), F32)
+            o.gemm(dt1pre, st.WT("t_embedder.mlp.0.weight"), dfreq, epi=EPI_F32)
+            dt = o.empty((B,), F32)
+            o.timestep_embed_bwd(dfreq, c.raw_t, dt)
+        if want_dy:  # y_embedder.y_proj.fc1 dgrad
+            wt = self._transposed("y_embedder.y_proj.fc1.weight")
+            dy = o.empty((da1pre.shape[0], wt.shape[0]), F32)
+            o.gemm(da1pre, wt, dy, epi=EPI_F32)
+        return dx, dt, dy
+
+    def _bwd_accumulators(self, c):
+        """dmod (grad wrt every adaLN vector) and dy2 (grad wrt the caption tokens: all cross-attentions + pooled path)."""
+        o = self.ops
+        return o.zeros(tuple(c.stem.mod.shape), F32), o.zeros((c.B * c.stem.L, self.cfg.dim), F32)
+
+    def _backward_from_tokens(self, c, dftok, dmod, dy2, grads_ready_hook=True, want_dx0=False, want_dt=False,
+                              want_dy=False):
+        """The backward shared by backward() and backward_output(), from d ftok (bf16 [B*Tk, p*p*C], the final-layer token
+        gradient) down to every parameter and the conditioning stem.  Returns (dx0b, dt1pre, da1pre): the bf16 gradients
+        at the patch-embed output, the timestep MLP's and the caption projection's pre-activations (None when not
+        computed; want_* only matter while weight gradients are skipped)."""
+        o, st, cfg = self.ops, self.store, self.cfg
+        P = st.p
         B, T, Tk = c.B, c.T, c.Tk
-        D, Dm, p = cfg.dim, cfg.mixer_dim, cfg.patch_size
+        D, Dm = cfg.dim, cfg.mixer_dim
         s = c.stem
         L = s.L
         mod = s.mod
-        dmod = o.zeros(tuple(mod.shape), F32)
-        dy2 = o.zeros((B * L, D), F32)  # grad wrt the caption tokens (all cross-attentions + pooled path)
-        # ---- loss -> final layer
-        dftok = o.empty((B * Tk, cfg.patch_dim), BF16)
-        o.edm_loss_bwd(c.ftok, c.keep_rows, c.lat, c.xn, c.coef, gscale, dftok, p, Tk)
-        o.colsum(dftok, G["final_layer.linear.bias"])
-        self._wgrad(dftok, c.xf, st.G("final_layer.linear.weight"))
+        self._colsum(dftok, self._gv("final_layer.linear.bias"))
+        self._wgrad(dftok, c.xf, self._Gv("final_layer.linear.weight"))
         dxf = o.empty((B * Tk, D), BF16)
         o.gemm(dftok, st.WT("final_layer.linear.weight"), dxf)
         fo = st.layout.ada_offset["final_layer"]
@@ -625,7 +711,7 @@ class Engine:
         fuse = self.fuse_ln and nb > 0 and cfg.blocks[-1].dim == D
         dy = o.empty((B * Tk, D), BF16) if fuse else None
         o.ln_bwd(dxf, c.xlast, c.m_f, c.r_f, gamma=P["final_layer.norm_final.weight"], scale=sc_f, T=Tk, dx=dx,
-                 dx_mode=0, dgamma=G["final_layer.norm_final.weight"], dshift=dmod[:, fo:fo + D],
+                 dx_mode=0, dgamma=self._gv("final_layer.norm_final.weight"), dshift=dmod[:, fo:fo + D],
                  dscale=dmod[:, fo + D:fo + 2 * D], dy_next=dy,
                  **(self._ffn_gate_args(cfg.blocks[-1], c.block_sv[-1], mod, dmod) if fuse else {}))
         # ---- backbone
@@ -637,7 +723,7 @@ class Engine:
             c.block_sv[i] = None  # release this block's saved activations
         self._kv_bwd("kv.blocks", dkv_b, s.ybf, dy2)
         del dkv_b
-        if self.on_backbone_grads_ready is not None:
+        if grads_ready_hook and self.on_backbone_grads_ready is not None:
             # every gradient of blocks.* / final_layer.* / the stacked kv.blocks is final from here on: the
             # data-parallel reducer can start moving ~3/4 of the bytes while the mixer and stem backward still run
             self.on_backbone_grads_ready()
@@ -645,13 +731,13 @@ class Engine:
         if cfg.has_mixer_maps:
             dxb = o.empty((B * Tk, D), BF16)
             o.gate_bwd(dx, dxb, T=Tk)
-            self._wgrad(dxb, c.xk_n, st.G("patch_mixer_map_xout.1.weight"))
+            self._wgrad(dxb, c.xk_n, self._Gv("patch_mixer_map_xout.1.weight"))
             dxk = o.empty((B * Tk, Dm), BF16)
             o.gemm(dxb, st.WT("patch_mixer_map_xout.1.weight"), dxk)
             dxm = o.zeros((B * T, Dm), F32)
             o.ln_bwd(dxk, c.xm_out, c.m_xo, c.r_xo, gamma=P["patch_mixer_map_xout.0.weight"], T=Tk,
                      src_rows=c.keep_rows, dx=dxm, dx_mode=2 if c.keep_rows is not None else 0,
-                     dgamma=G["patch_mixer_map_xout.0.weight"])
+                     dgamma=self._gv("patch_mixer_map_xout.0.weight"))
         elif c.keep_rows is not None:
             dxm = o.zeros((B * T, dx.shape[1]), F32)
             o.scatter_rows(dx, c.keep_rows, dxm)
@@ -674,31 +760,35 @@ class Engine:
                 # caption map: y_mixer = Linear(LN(y))
                 dymb = o.empty((B * L, Dm), BF16)
                 o.gate_bwd(dymix, dymb, T=L)
-                self._wgrad(dymb, c.y_n, st.G("patch_mixer_map_y.1.weight"))
+                self._wgrad(dymb, c.y_n, self._Gv("patch_mixer_map_y.1.weight"))
                 dyn = o.empty((B * L, D), BF16)
                 o.gemm(dymb, st.WT("patch_mixer_map_y.1.weight"), dyn)
                 o.ln_bwd(dyn, s.y2, c.m_y, c.r_y, gamma=P["patch_mixer_map_y.0.weight"], T=L, dx=dy2, dx_mode=0,
-                         dgamma=G["patch_mixer_map_y.0.weight"])
+                         dgamma=self._gv("patch_mixer_map_y.0.weight"))
                 # token map: x_mixer = Linear(LN(x0))
                 dxmb = o.empty((B * T, Dm), BF16)
                 o.gate_bwd(dxm, dxmb, T=T)
-                self._wgrad(dxmb, c.xin_n, st.G("patch_mixer_map_xin.1.weight"))
+                self._wgrad(dxmb, c.xin_n, self._Gv("patch_mixer_map_xin.1.weight"))
                 dxn = o.empty((B * T, D), BF16)
                 o.gemm(dxmb, st.WT("patch_mixer_map_xin.1.weight"), dxn)
                 dx0 = o.zeros((B * T, D), F32)
                 o.ln_bwd(dxn, c.x0, c.m_xin, c.r_xin, gamma=P["patch_mixer_map_xin.0.weight"], T=T, dx=dx0, dx_mode=0,
-                         dgamma=G["patch_mixer_map_xin.0.weight"])
+                         dgamma=self._gv("patch_mixer_map_xin.0.weight"))
             else:
                 dx0 = dxm
         else:
             dx0 = dxm
-        # ---- patch embed (input is data: weight / bias gradients only)
-        dx0b = o.empty(tuple(dx0.shape), BF16)
-        o.gate_bwd(dx0, dx0b, T=T)
-        o.colsum(dx0, G["x_embedder.proj.bias"])
-        self._wgrad(dx0b, c.patches, st.G("x_embedder.proj.weight"))
+        # ---- patch embed
+        dx0b = None
+        if want_dx0 or not self._skip_wgrad:
+            dx0b = o.empty(tuple(dx0.shape), BF16)
+            o.gate_bwd(dx0, dx0b, T=T)
+        self._colsum(dx0, self._gv("x_embedder.proj.bias"))
+        self._wgrad(dx0b, c.patches, self._Gv("x_embedder.proj.weight"))
         # ---- conditioning stem
-        self._stem_bwd(s, dmod, dy2, B)
+        if want_dt or want_dy or not self._skip_wgrad:
+            return (dx0b, *self._stem_bwd(s, dmod, dy2, B, want_dt, want_dy))
+        return dx0b, None, None
 
     # buffers owned by the nn.Module (pos_embed / mask_token), attached by models.dit.DiT
     pos_embed: Optional[torch.Tensor] = None

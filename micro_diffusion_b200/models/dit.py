@@ -3,9 +3,10 @@
 Same constructor arguments, attribute names, factories and state_dict (476 parameters + `pos_embed`,
 `mask_token`; SURVEY.md section 8b) as reference micro_diffusion/models/dit.py, but the module holds no
 compute: parameters are views into one flat fp32 buffer (`params.ParamStore`) and `forward` hands raw
-device pointers to the sm_90a kernels through `engine.Engine`.  Training gradients come from the
-hand-written backward driven by `LatentDiffusion.forward` (models/model.py), not from autograd through
-this module; calling `DiT.forward` directly is the inference entry (no_grad) the sampler uses.
+device pointers to the sm_90a kernels through `engine.Engine`.  Gradients come from the hand-written CUDA
+backward: `LatentDiffusion.forward` drives it for the fused EDM loss (models/model.py), and `DiT.forward` under grad
+mode records one autograd node (`_DiTForwardFn`) whose backward runs the same backward from an arbitrary output
+cotangent and returns the gradients of x, t and y.  Under no_grad `DiT.forward` is the plain inference entry.
 """
 from __future__ import annotations
 
@@ -13,6 +14,7 @@ from typing import List, Optional
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from ..arch import DiTConfig, micro_dit_tiny_2_kwargs, micro_dit_xl_2_kwargs
 from ..engine import Engine
@@ -38,6 +40,41 @@ def _trunc_normal_(t: torch.Tensor, std: float, gen=None):
     # but keep the semantics.
     with torch.no_grad():
         t.normal_(0.0, std, generator=gen).clamp_(-2.0, 2.0)
+
+
+class _DiTForwardFn(torch.autograd.Function):
+    """F = DiT.forward_without_cfg(x, t, y)["sample"] with the forward and its vector-Jacobian product run by the engine.
+
+    `anchor` is the DiT's gradient anchor when parameter gradients are wanted (they accumulate into the flat buffer behind
+    `p.grad`, like the fused loss) and None when every parameter is frozen.  x f32 and t f32 [B] arrive already cast and
+    broadcast by the caller, so autograd handles those; the fp16 storage cast of y happens in here and its gradient is
+    returned in y's own dtype (a straight-through cast, without rounding the gradient to fp16)."""
+
+    @staticmethod
+    def forward(ctx, anchor, dit, x, t, y, mask_ratio, mask_noise):
+        fx, mask, c = dit.engine.forward_raw(x, t, dit._caption_f16(y), mask_ratio, mask_noise, keep=True)
+        ctx.dit, ctx.c, ctx.param_grads = dit, c, anchor is not None
+        ctx.y_shape, ctx.y_dtype = y.shape, y.dtype
+        if mask is not None:
+            ctx.mark_non_differentiable(mask)
+        return fx, mask
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dfx, dmask=None):
+        dit, c = ctx.dit, ctx.c
+        if c is None:
+            raise RuntimeError("DiT backward: no saved activations (backward called twice through the same forward)")
+        want_dx, want_dt, want_dy = ctx.needs_input_grad[2:5]
+        if ctx.param_grads:
+            dit.prepare_grads()
+        dF = dfx.detach().to(torch.float32).contiguous()
+        dx, dt, dy = dit.engine.backward_output(c, dF, param_grads=ctx.param_grads, want_dx=want_dx, want_dt=want_dt,
+                                                want_dy=want_dy)
+        ctx.c = None  # free the saved activations
+        if dy is not None:
+            dy = dy.reshape(ctx.y_shape).to(ctx.y_dtype)
+        return None, None, dx, dt, dy, None, None
 
 
 class DiT(nn.Module):
@@ -228,9 +265,28 @@ class DiT(nn.Module):
             P["final_layer.adaLN_modulation.1.weight"].zero_()
             P["final_layer.linear.weight"].zero_()
 
-    # ------------------------------------------------------------------ inference entry (dit.py:455-564)
-    @torch.no_grad()
+    # ------------------------------------------------------------------ forward (dit.py:455-564)
     def forward_without_cfg(self, x, t, y, mask_ratio: float = 0, **kwargs) -> dict:
+        """Differentiable like the reference's: under grad mode, when x, t, y or the parameters require grad, the output
+        carries one autograd node whose backward is the engine's hand-derived backward.  Otherwise (e.g. under no_grad)
+        nothing is saved."""
+        if torch.is_grad_enabled():
+            param_grads = self._param_grad_mode()
+            if param_grads or any(torch.is_tensor(v) and v.requires_grad for v in (x, t, y)):
+                self.engine  # bind storage / anchor before the autograd node is built
+                B = x.shape[0]
+                x = x.float().contiguous()
+                t = t.float().reshape(-1).expand(B).contiguous()
+                noise = None
+                if mask_ratio > 0:
+                    noise = torch.rand(B, self.cfg.num_patches, device=x.device)  # get_mask (utils.py:390)
+                fx, mask = _DiTForwardFn.apply(self._anchor if param_grads else None, self, x, t, y, float(mask_ratio),
+                                               noise)
+                return {"sample": fx, "mask": mask}
+        return self._forward_inference(x, t, y, mask_ratio)
+
+    @torch.no_grad()
+    def _forward_inference(self, x, t, y, mask_ratio):
         eng = self.engine
         B = x.shape[0]
         x = x.float().contiguous()
@@ -242,7 +298,15 @@ class DiT(nn.Module):
         fx, mask = eng.forward_raw(x, t, cap, mask_ratio, noise)
         return {"sample": fx, "mask": mask}
 
-    @torch.no_grad()
+    def _param_grad_mode(self) -> bool:
+        """True when every parameter requires grad, False when none does; per-parameter freezing is not supported."""
+        req = {p.requires_grad for p in self.parameters()}
+        if len(req) > 1:
+            raise NotImplementedError("DiT: some parameters require grad and some do not. The CUDA backward computes the "
+                                      "gradients of all parameters or of none: set requires_grad on all of them, or on "
+                                      "none (input gradients only).")
+        return req.pop()
+
     def forward_with_cfg(self, x, t, y, cfg: float = 1.0, mask_ratio: float = 0, **kwargs) -> dict:
         x = torch.cat([x, x], 0)
         y = torch.cat([y, torch.zeros_like(y)], 0)
@@ -253,9 +317,6 @@ class DiT(nn.Module):
         return {"sample": uncond_eps + cfg * (cond_eps - uncond_eps)}
 
     def forward(self, x, t, y, cfg: float = 1.0, **kwargs) -> dict:
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()) and self.training:
-            raise RuntimeError("DiT.forward is the inference entry; training gradients are produced by "
-                               "LatentDiffusion.forward (the fused EDM loss path). Wrap the call in torch.no_grad().")
         if cfg != 1.0:
             return self.forward_with_cfg(x, t, y, cfg, **kwargs)
         return self.forward_without_cfg(x, t, y, **kwargs)

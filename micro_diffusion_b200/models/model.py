@@ -165,9 +165,10 @@ class LatentDiffusion(_Base):
         return self._edm_loss_impl(x, y, None, mask_ratio)
 
     def model_forward_wrapper(self, x, sigma, y, model_forward_fxn, mask_ratio: float, **kwargs) -> dict:
-        """EDM preconditioning around the denoiser (model.py:144-179).  The fused kernel path is taken when
-        `model_forward_fxn` is this model's own DiT (plain or CFG partial); anything else gets the generic
-        composition with the caller's function."""
+        """EDM preconditioning around the denoiser (model.py:144-179).  The fused kernel path (no gradients) is taken
+        when `model_forward_fxn` is this model's own DiT (plain or CFG partial) and no gradient is wanted; under grad
+        mode with x, sigma, y or a DiT parameter requiring grad, and for any other function, the reference's own
+        composition c_skip*x + c_out*F(c_in*x, ln(sigma)/4, y) runs over the (differentiable) DiT.forward."""
         fn, cfg = model_forward_fxn, 1.0
         if isinstance(fn, partial) and getattr(fn.func, "__self__", None) is self.dit:
             cfg = fn.keywords.get("cfg", 1.0)
@@ -175,7 +176,8 @@ class LatentDiffusion(_Base):
         own = fn is self.dit or getattr(fn, "__self__", None) is self.dit
         B = x.shape[0]
         sigma_b = sigma.to(torch.float32).reshape(-1).expand(B).contiguous()
-        if own and not (torch.is_grad_enabled() and self.dit.training and mask_ratio > 0):
+        fused = own and not self._wants_grad(x, sigma, y)
+        if fused and not (torch.is_grad_enabled() and self.dit.training and mask_ratio > 0):
             with torch.no_grad():
                 eng = self.dit.engine
                 xin = x.float().contiguous()
@@ -212,6 +214,13 @@ class LatentDiffusion(_Base):
         out = model_forward_fxn((c_in * x).to(x.dtype), (sg.log() / 4).flatten(), y, mask_ratio=mask_ratio, **kwargs)
         out["sample"] = c_skip * x + c_out * out["sample"]
         return out
+
+    def _wants_grad(self, x, sigma, y) -> bool:
+        """Grad mode is on and a gradient is wanted for an input or for the DiT's parameters."""
+        if not torch.is_grad_enabled():
+            return False
+        return (any(torch.is_tensor(v) and v.requires_grad for v in (x, sigma, y))
+                or any(p.requires_grad for p in self.dit.parameters()))
 
     # ------------------------------------------------------------------ Composer hooks (model.py:213-229)
     def loss(self, outputs: tuple, batch: dict) -> torch.Tensor:

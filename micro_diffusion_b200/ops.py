@@ -67,6 +67,9 @@ _PROTOS = {
     "md_edm_loss_fwd": [_P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _P],
     "md_edm_loss_bwd": [_P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _I, _P],
     "md_edm_output": [_P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _P],
+    "md_unpatchify_bwd": [_P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _I, _P],
+    "md_patchify_bwd": [_P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I, _P],
+    "md_timestep_embed_bwd": [_P, _P, _P, _I64, _I64, _I, _P],
     "md_mean_tokens_fwd": [_P, _P, _I64, _I64, _I64, _I, _P],
     "md_mean_tokens_bwd": [_P, _P, _I64, _I64, _I64, _P],
     "md_cast_f32_bf16": [_P, _P, _I64, _I, _P],
@@ -78,7 +81,7 @@ _PROTOS = {
     "md_adamw": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _F, _F, _I64, _P, _I64, _P],
 }
 
-_TAKES_PREC = frozenset(['md_ln_fwd', 'md_ln_bwd', 'md_rownorm_fwd', 'md_rownorm_bwd', 'md_gate_bwd', 'md_swiglu_fwd', 'md_swiglu_bwd', 'md_act_fwd', 'md_act_bwd', 'md_gelu_tanh_f32_fwd', 'md_moe_gate_fwd', 'md_moe_gather', 'md_moe_combine_fwd', 'md_moe_combine_bwd', 'md_moe_dx_bwd', 'md_moe_gate_wgrad', 'md_cond_prepare', 'md_edm_prepare', 'md_patchify', 'md_timestep_embed', 'md_edm_loss_bwd', 'md_mean_tokens_fwd', 'md_cast_f32_bf16', 'md_cast_transpose', 'md_cast_transpose_multi'])
+_TAKES_PREC = frozenset(['md_ln_fwd', 'md_ln_bwd', 'md_rownorm_fwd', 'md_rownorm_bwd', 'md_gate_bwd', 'md_swiglu_fwd', 'md_swiglu_bwd', 'md_act_fwd', 'md_act_bwd', 'md_gelu_tanh_f32_fwd', 'md_moe_gate_fwd', 'md_moe_gather', 'md_moe_combine_fwd', 'md_moe_combine_bwd', 'md_moe_dx_bwd', 'md_moe_gate_wgrad', 'md_cond_prepare', 'md_edm_prepare', 'md_patchify', 'md_timestep_embed', 'md_edm_loss_bwd', 'md_unpatchify_bwd', 'md_patchify_bwd', 'md_timestep_embed_bwd', 'md_mean_tokens_fwd', 'md_cast_f32_bf16', 'md_cast_transpose', 'md_cast_transpose_multi'])
 
 EXPORTED_SYMBOLS = ["md_last_error", "md_abi_version", "md_gemm_bf16", *_PROTOS.keys()]
 
@@ -464,6 +467,25 @@ class CudaOps:
         B, Cc, H, W = ref.shape
         self._call("md_edm_output", ftok.data_ptr(), _ptr(ids_restore), _ptr(mask_token), _ptr(xn), _ptr(coef),
                    _ptr(fx), _ptr(dx), B, Cc, H, W, p, Tk)
+
+    # ------------------------------------------------------------------ adjoints of the DiT input / output maps
+    def unpatchify_bwd(self, dF, keep_rows, dftok, p, Tk):
+        """dftok [B*Tk, p*p*C] = adjoint of edm_output's un-mask + unpatchify at the kept tokens (all when keep_rows is None)."""
+        B, Cc, H, W = dF.shape
+        assert dF.is_contiguous() and dF.dtype == torch.float32 and dftok.shape == (B * Tk, p * p * Cc)
+        self._call("md_unpatchify_bwd", dF.data_ptr(), _ptr(keep_rows), dftok.data_ptr(), B, Cc, H, W, p, Tk)
+
+    def patchify_bwd(self, dpatches, scale, dx, p):
+        """dx f32 [B,C,H,W] = adjoint of patchify (col2im) of dpatches f32 [B*T, C*p*p]."""
+        B, Cc, H, W = dx.shape
+        assert dpatches.is_contiguous() and dpatches.dtype == torch.float32 and dx.is_contiguous()
+        assert dpatches.shape == (B * (H // p) * (W // p), Cc * p * p)
+        self._call("md_patchify_bwd", dpatches.data_ptr(), _ptr(scale), dx.data_ptr(), B, Cc, H, W, p)
+
+    def timestep_embed_bwd(self, dfreq, t, dt):
+        """dt f32 [B] = adjoint of timestep_embed at t for the cotangent dfreq f32 [B, dim]."""
+        assert dfreq.is_contiguous() and dfreq.dtype == torch.float32 and t.dtype == torch.float32 and t.is_contiguous()
+        self._call("md_timestep_embed_bwd", dfreq.data_ptr(), t.data_ptr(), dt.data_ptr(), dfreq.shape[0], dfreq.shape[1])
 
     # ------------------------------------------------------------------ utilities
     def mean_tokens_fwd(self, x, out, B, L):
