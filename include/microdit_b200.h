@@ -64,10 +64,13 @@ MD_API int md_set_deterministic(void* workspace, int64_t bytes);
 #define MD_EPI_ACT_GRAD 5   /* C(bf16) = alpha*acc * act'(aux) (no bias): the dgrad GEMM of an activation's output applies the
                              * activation's derivative at the saved pre-activation aux (bf16, indexed like C) */
 
-#define MD_EPI_SWIGLU 6     /* N = 2f columns in the 32-interleaved order (w1 block j, w2 block j, ...): C(bf16) = u = alpha*acc,
-                             * C2(bf16 [M, f], pitch ldc2) = silu(u1) * u2 (FeedForward, dit.py:88-89) */
+#define MD_EPI_SWIGLU 6     /* N = 2f columns in the 32-interleaved order (w1 block j, w2 block j, ...): C(bf16) = u = alpha*acc
+                             * (+bias), C2(bf16 [M, f], pitch ldc2) = silu(u1) * u2 (FeedForward, dit.py:84-89).  bias (optional,
+                             * f32 [batch][2f]) is in the natural [b1 | b2] order: interleaved column c = 64 j + r takes
+                             * bias[32 j + r] for r < 32 and bias[f + 32 j + r - 32] otherwise, and is added before u is
+                             * rounded and stored, so the u that MD_EPI_SWIGLU_GRAD reads back includes it */
 #define MD_EPI_SWIGLU_GRAD 7 /* N = f: acc = d h; C(bf16 [M, 2f] interleaved) = (d h * u2 * silu'(u1) | d h * silu(u1)) with
-                              * u = aux (bf16 [M, 2f] interleaved, indexed like C) */
+                              * u = aux (bf16 [M, 2f] interleaved, indexed like C); no bias */
 
 typedef struct md_gemm_args {
   const void* A; /* bf16 */
@@ -303,6 +306,12 @@ MD_API int md_mean_tokens_bwd(const float* d, float* dx, int64_t B, int64_t L, i
 MD_API int md_cast_f32_bf16(const float* x, void* y, int64_t n, int prec, void* stream);
 /* out(f32 [N]) += column sums of x [rows, N] (bf16 if x_bf16 else f32), pitch ld (bias gradients) */
 MD_API int md_colsum(const void* x, int x_bf16, int64_t ld, float* out, int64_t rows, int64_t N, void* stream);
+/* The same for a fused-SwiGLU gradient du [rows, N = 2 half] in the 32-interleaved column order of MD_EPI_SWIGLU
+ * (half % 32 == 0): out(f32 [2 half]) += the column sums in the natural [b1 | b2] order -- column c = 64 j + r goes to
+ * 32 j + r (r < 32) or half + 32 j + r - 32, the row map of md_gemm_args.row_interleave -- i.e. the bias gradient of
+ * a w1 | w2 stack (dit.py:84-86 with use_bias).  Deterministic mode as md_colsum. */
+MD_API int md_colsum_interleaved(const void* x, int x_bf16, int64_t ld, float* out, int64_t rows, int64_t N, int64_t half,
+                                 void* stream);
 /* W f32 [batch, rows, cols] -> wb bf16 same layout (optional) and wbt bf16 [batch, cols, rows] (optional):
  * the per-step bf16 operand copies of the fp32 master weights (what autocast does per call in the reference).
  * interleave_half = f > 0 (rows == 2f, f % 32 == 0): both copies hold the rows in the 32-interleaved order of the fused

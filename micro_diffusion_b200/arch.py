@@ -127,25 +127,29 @@ class DiTConfig:
         return [*self.mixer_blocks, *self.blocks]
 
     # ------------------------------------------------------------------ parameter list
+    def _linear(self, name: str, out_f: int, in_f: int) -> List[Tuple[str, Tuple[int, ...]]]:
+        """nn.Linear(in_f, out_f, bias=use_bias): the weight, then its bias when the model has biases."""
+        return [(name + ".weight", (out_f, in_f))] + ([(name + ".bias", (out_f,))] if self.use_bias else [])
+
     def block_param_specs(self, b: BlockSpec) -> List[Tuple[str, Tuple[int, ...]]]:
         D, h, f, E = b.dim, b.attn_dim, b.ffn_dim, self.num_experts
-        p = b.name
-        out = [(f"{p}.norm1.weight", (D,)), (f"{p}.attn.qkv.weight", (3 * h, D)), (f"{p}.attn.proj.weight", (D, h)),
-               (f"{p}.cross_attn.q_linear.weight", (D, D)), (f"{p}.cross_attn.kv_linear.weight", (2 * D, D)),
-               (f"{p}.cross_attn.proj.weight", (D, D)), (f"{p}.norm2.weight", (D,)), (f"{p}.norm3.weight", (D,))]
-        if b.moe:
+        p, lin = b.name, self._linear
+        out = [(f"{p}.norm1.weight", (D,)), *lin(f"{p}.attn.qkv", 3 * h, D), *lin(f"{p}.attn.proj", D, h),
+               *lin(f"{p}.cross_attn.q_linear", D, D), *lin(f"{p}.cross_attn.kv_linear", 2 * D, D),
+               *lin(f"{p}.cross_attn.proj", D, D), (f"{p}.norm2.weight", (D,)), (f"{p}.norm3.weight", (D,))]
+        if b.moe:  # the expert banks are raw parameters and the gate is bias-free whatever use_bias says (dit.py:107-124)
             out += [(f"{p}.mlp.w1", (E, D, f)), (f"{p}.mlp.w2", (E, f, D)), (f"{p}.mlp.gate.weight", (E, D))]
         else:
-            out += [(f"{p}.mlp.w1.weight", (f, D)), (f"{p}.mlp.w2.weight", (f, D)), (f"{p}.mlp.w3.weight", (D, f))]
+            out += [*lin(f"{p}.mlp.w1", f, D), *lin(f"{p}.mlp.w2", f, D), *lin(f"{p}.mlp.w3", D, f)]
         out += [(f"{p}.adaLN_modulation.1.weight", (6 * D, self.dim)), (f"{p}.adaLN_modulation.1.bias", (6 * D,))]
         return out
 
     def param_specs(self) -> List[Tuple[str, Tuple[int, ...]]]:
-        """(name, shape) of every trainable parameter, in the reference's state_dict order."""
-        if self.use_bias:
-            raise NotImplementedError("use_bias=True is not on the MicroDiT path (both zoo models pass use_bias=False, "
-                                      "dit.py:664,705); only the bias-free block linears are implemented")
+        """(name, shape) of every trainable parameter, in the reference's state_dict order.  use_bias=True adds the bias
+        of every block linear, of the prompt block's attention / SwiGLU and of the mixer maps (dit.py:39-51,84-86,202-219,
+        377-388), each right after its weight."""
         D, C, p, Dc = self.dim, self.in_channels, self.patch_size, self.caption_channels
+        lin = self._linear
         fp = self.prompt_ffn_dim
         s: List[Tuple[str, Tuple[int, ...]]] = [
             ("x_embedder.proj.weight", (D, C, p, p)), ("x_embedder.proj.bias", (D,)),
@@ -154,10 +158,10 @@ class DiTConfig:
             ("y_embedder.y_proj.fc1.weight", (D, Dc)), ("y_embedder.y_proj.fc1.bias", (D,)),
             ("y_embedder.y_proj.norm.weight", (D,)),
             ("y_embedder.y_proj.fc2.weight", (D, D)), ("y_embedder.y_proj.fc2.bias", (D,)),
-            ("y_emb_preprocess.norm1.weight", (D,)), ("y_emb_preprocess.attn.qkv.weight", (3 * D, D)),
-            ("y_emb_preprocess.attn.proj.weight", (D, D)), ("y_emb_preprocess.norm2.weight", (D,)),
-            ("y_emb_preprocess.mlp.w1.weight", (fp, D)), ("y_emb_preprocess.mlp.w2.weight", (fp, D)),
-            ("y_emb_preprocess.mlp.w3.weight", (D, fp)),
+            ("y_emb_preprocess.norm1.weight", (D,)), *lin("y_emb_preprocess.attn.qkv", 3 * D, D),
+            *lin("y_emb_preprocess.attn.proj", D, D), ("y_emb_preprocess.norm2.weight", (D,)),
+            *lin("y_emb_preprocess.mlp.w1", fp, D), *lin("y_emb_preprocess.mlp.w2", fp, D),
+            *lin("y_emb_preprocess.mlp.w3", D, fp),
             ("pooled_y_emb_process.fc1.weight", (D, D)), ("pooled_y_emb_process.fc1.bias", (D,)),
             ("pooled_y_emb_process.norm.weight", (D,)),
             ("pooled_y_emb_process.fc2.weight", (D, D)), ("pooled_y_emb_process.fc2.bias", (D,)),
@@ -166,9 +170,9 @@ class DiTConfig:
             s += self.block_param_specs(b)
         if self.has_mixer_maps:
             Dm = self.patch_mixer_dim
-            s += [("patch_mixer_map_xin.0.weight", (D,)), ("patch_mixer_map_xin.1.weight", (Dm, D)),
-                  ("patch_mixer_map_xout.0.weight", (Dm,)), ("patch_mixer_map_xout.1.weight", (D, Dm)),
-                  ("patch_mixer_map_y.0.weight", (D,)), ("patch_mixer_map_y.1.weight", (Dm, D))]
+            s += [("patch_mixer_map_xin.0.weight", (D,)), *lin("patch_mixer_map_xin.1", Dm, D),
+                  ("patch_mixer_map_xout.0.weight", (Dm,)), *lin("patch_mixer_map_xout.1", D, Dm),
+                  ("patch_mixer_map_y.0.weight", (D,)), *lin("patch_mixer_map_y.1", Dm, D)]
         for b in self.blocks:
             s += self.block_param_specs(b)
         s += [("final_layer.linear.weight", (self.patch_dim, D)), ("final_layer.linear.bias", (self.patch_dim,)),

@@ -151,10 +151,18 @@ __global__ void copy_f32_kernel(const float* __restrict__ x, float* __restrict__
 
 // ------------------------------------------------------------------------------------------ colsum
 // grid (ceil(N/256), ceil(rows/256)): each thread owns one column of a 256-row slab.
+// half > 0: x holds the 2 half columns of a fused-SwiGLU output in the 32-interleaved order (u1 block j, u2 block j, ...);
+// column c = 64 j + r lands at 32 j + r (r < 32, b1) or half + 32 j + r - 32 (b2) of out, the [b1 | b2] order.
+template <bool kInterleaved>
 __global__ void colsum_kernel(const void* __restrict__ x, int x_bf16, long long ld, float* __restrict__ out,
-                              long long rows, long long N, float* __restrict__ ws) {
+                              long long rows, long long N, float* __restrict__ ws, long long half) {
   const long long c = 1LL * blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= N) return;
+  long long oc = c;
+  if constexpr (kInterleaved) {
+    const long long j = c >> 6, r = c & 63;
+    oc = (r < 32 ? 0 : half - 32) + 32 * j + r;
+  }
   const long long r0 = 1LL * blockIdx.y * 256, r1 = min(rows, r0 + 256);
   float s = 0.f;
   if (x_bf16) {
@@ -164,8 +172,8 @@ __global__ void colsum_kernel(const void* __restrict__ x, int x_bf16, long long 
     const float* p = reinterpret_cast<const float*>(x);
     for (long long r = r0; r < r1; ++r) s += p[r * ld + c];
   }
-  if (ws != nullptr) ws[1LL * blockIdx.y * N + c] = s;   // deterministic mode: slab partials, fixed-order reduction afterwards
-  else atomicAdd(out + c, s);
+  if (ws != nullptr) ws[1LL * blockIdx.y * N + oc] = s;   // deterministic mode: slab partials, fixed-order reduction afterwards
+  else atomicAdd(out + oc, s);
 }
 
 // ---------------------------------------------------------------------------------- cast_transpose
@@ -444,8 +452,24 @@ extern "C" int md_colsum(const void* x, int x_bf16, int64_t ld, float* out, int6
     ws = det_workspace(static_cast<size_t>(grid.y) * N * sizeof(float));
     if (ws == nullptr) return md_set_error(MD_ERR_INVALID, "md_colsum: deterministic workspace too small");
   }
-  colsum_kernel<<<grid, 256, 0, ST(stream)>>>(x, x_bf16, ld, out, rows, N, ws);
+  colsum_kernel<false><<<grid, 256, 0, ST(stream)>>>(x, x_bf16, ld, out, rows, N, ws, 0);
   if (int rc = check_launch("md_colsum")) return rc;
+  return ws ? det_reduce(ws, out, grid.y, N, 1, ST(stream)) : 0;
+}
+extern "C" int md_colsum_interleaved(const void* x, int x_bf16, int64_t ld, float* out, int64_t rows, int64_t N,
+                                     int64_t half, void* stream) {
+  if (rows == 0 || N == 0) return 0;
+  if (!x || !out) return md_set_error(MD_ERR_INVALID, "md_colsum_interleaved: null pointer");
+  if (half <= 0 || half % 32 != 0 || N != 2 * half)
+    return md_set_error(MD_ERR_INVALID, "md_colsum_interleaved: needs N == 2 half and half % 32 == 0");
+  dim3 grid((unsigned)((N + 255) / 256), (unsigned)((rows + 255) / 256));
+  float* ws = nullptr;
+  if (det_enabled()) {
+    ws = det_workspace(static_cast<size_t>(grid.y) * N * sizeof(float));
+    if (ws == nullptr) return md_set_error(MD_ERR_INVALID, "md_colsum_interleaved: deterministic workspace too small");
+  }
+  colsum_kernel<true><<<grid, 256, 0, ST(stream)>>>(x, x_bf16, ld, out, rows, N, ws, half);
+  if (int rc = check_launch("md_colsum_interleaved")) return rc;
   return ws ? det_reduce(ws, out, grid.y, N, 1, ST(stream)) : 0;
 }
 extern "C" int md_cast_transpose(const float* w, void* wb, void* wbt, int64_t batch, int64_t rows, int64_t cols,

@@ -385,10 +385,20 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // 32 rows (w1 block j, w2 block j, ...), so column c < 32 of every 64-column group holds u1 and column c + 32 the
         // matching u2 -- register pairs j and j + 4 of the same thread: C = u (bf16, the interleaved layout backward reads
         // again), C2 = silu(u1) * u2 (bf16, natural layout).  N % 64 == 0 and 32-byte aligned outputs (host-checked).
+        // The optional bias is the natural-order [b1 | b2] fp32 vector: u1 column col (col % 64 < 32) takes
+        // b1[32 (col / 64) + col % 64], its u2 partner b2 at the same index; u = acc + b is what C keeps for backward.
         for_each_pair([&](int row, long long crow, int i, int j, int col, float, float, bool) {
           if ((j & 7) >= 4) return;
-          const float a0 = bf16_round(acc[4 * j + 2 * i] * alpha), a1 = bf16_round(acc[4 * j + 2 * i + 1] * alpha);
-          const float b0 = bf16_round(acc[4 * (j + 4) + 2 * i] * alpha), b1 = bf16_round(acc[4 * (j + 4) + 2 * i + 1] * alpha);
+          float a0 = acc[4 * j + 2 * i] * alpha, a1 = acc[4 * j + 2 * i + 1] * alpha;
+          float b0 = acc[4 * (j + 4) + 2 * i] * alpha, b1 = acc[4 * (j + 4) + 2 * i + 1] * alpha;
+          if (p.bias != nullptr) {
+            const float* bb = p.bias + 1LL * bz * p.strideBias + 32 * (col >> 6) + (col & 63);
+            const float2 x1 = ld_f32_pair(bb, true, vec), x2 = ld_f32_pair(bb + (p.N >> 1), true, vec);
+            a0 += x1.x; a1 += x1.y;
+            b0 += x2.x; b1 += x2.y;
+          }
+          a0 = bf16_round(a0); a1 = bf16_round(a1);
+          b0 = bf16_round(b0); b1 = bf16_round(b1);
           __nv_bfloat16* du = reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col;
           st_bf16_pair(du, a0, a1, true, true);
           st_bf16_pair(du + 32, b0, b1, true, true);
@@ -512,8 +522,9 @@ extern "C" int md_gemm_bf16(const md_gemm_args* a, void* stream_) {
     const bool fwd = a->epilogue == EPI_SWIGLU;
     const void* second = fwd ? a->C2 : a->aux;
     const int64_t ld2 = fwd ? (a->ldc2 > 0 ? a->ldc2 : a->N / 2) : a->ldc;
-    if (second == nullptr || a->bias != nullptr || a->layout != MD_GEMM_NT || a->splits > 1)
-      return md_set_error(MD_ERR_INVALID, "md_gemm_bf16: SwiGLU epilogues need C2 (forward) / aux (backward), NT layout, no bias");
+    if (second == nullptr || (!fwd && a->bias != nullptr) || a->layout != MD_GEMM_NT || a->splits > 1)
+      return md_set_error(MD_ERR_INVALID,
+                          "md_gemm_bf16: SwiGLU epilogues need C2 (forward) / aux (backward), NT layout, no bias on the backward");
     if (a->N % (fwd ? 64 : 32) != 0 || (a->ldc % 16) != 0 || (ld2 % 16) != 0 ||
         ((reinterpret_cast<uintptr_t>(a->C) | reinterpret_cast<uintptr_t>(second)) & 31) != 0 ||
         (a->batch > 1 && ((a->strideC % 16) != 0 || (fwd && (a->strideC2 % 16) != 0))))

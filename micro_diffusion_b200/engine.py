@@ -54,6 +54,16 @@ class Engine:
         if out is not None:
             self.ops.colsum(x, out)
 
+    def _bkw(self, key):
+        """{"bias": fp32 bias} of a use_bias Linear / stacked group (ParamStore.bias), {} when it has none: a bias-free model
+        issues its GEMMs with exactly the arguments it always did."""
+        b = self.store.bias(key)
+        return {} if b is None else {"bias": b}
+
+    def _gb(self, key):
+        """Gradient view of the bias of a Linear / stacked group, or None (no bias, or weight gradients skipped)."""
+        return None if self._skip_wgrad else self.store.gbias(key)
+
     def _wgrad(self, dY, X, G):
         """G[P,Q] (+)= dY[r,P]^T X[r,Q]  (reduction over the rows r); the library picks the split of the
         reduction that fills the SMs (splits=0).  Skipped when G is None."""
@@ -76,24 +86,33 @@ class Engine:
         return wt
 
     def _swiglu_fwd(self, name_w12, x, u, hact):
-        """u = x W12^T, hact = silu(u1) * u2 (dit.py:88-89): one GEMM when the stack is interleaved, GEMM + pass otherwise."""
+        """u = x W12^T (+ [b1 | b2]), hact = silu(u1) * u2 (dit.py:88-89): one GEMM when the stack is interleaved (the
+        epilogue maps the natural-order bias onto the interleaved columns), GEMM + pass otherwise."""
         o, st = self.ops, self.store
         if st.interleave.get(name_w12, 0):
-            o.gemm(x, st.W(name_w12), u, epi=EPI_SWIGLU, C2=hact)
+            o.gemm(x, st.W(name_w12), u, epi=EPI_SWIGLU, C2=hact, **self._bkw(name_w12))
         else:
-            o.gemm(x, st.W(name_w12), u)
+            o.gemm(x, st.W(name_w12), u, **self._bkw(name_w12))
             o.swiglu_fwd(u, hact)
 
     def _swiglu_bwd(self, name_w12, name_w3, dy, u, du):
-        """du = d(silu(u1) * u2) for d hact = dy W3: inside the w3 dgrad GEMM when the stack is interleaved."""
+        """du = d(silu(u1) * u2) for d hact = dy W3: inside the w3 dgrad GEMM when the stack is interleaved.  With biases,
+        also the bias gradient of w1 | w2: the column sums of du, in [b1 | b2] order."""
         o, st = self.ops, self.store
         f = u.shape[1] // 2
-        if st.interleave.get(name_w12, 0):
+        half = st.interleave.get(name_w12, 0)
+        if half:
             o.gemm(dy, st.WT(name_w3), du, epi=EPI_SWIGLU_GRAD, aux=u)
         else:
             dh = o.empty((dy.shape[0], f), BF16)
             o.gemm(dy, st.WT(name_w3), dh)
             o.swiglu_bwd(dh, u, du)
+        g12 = self._gb(name_w12)
+        if g12 is not None:
+            if half:
+                o.colsum_interleaved(du, g12, half)
+            else:
+                o.colsum(du, g12)
 
     def _mods(self, key, D, mod):
         o = self.store.layout.ada_offset[key]
@@ -104,12 +123,13 @@ class Engine:
         """kv_linear of every block of a stage in one GEMM: [B*L, Dy] x [nblk*2D, Dy]^T (utils.py:118)."""
         o, st = self.ops, self.store
         kv_all = o.empty((ykv.shape[0], nblk * D2), BF16)
-        o.gemm(ykv, st.W(group), kv_all)
+        o.gemm(ykv, st.W(group), kv_all, **self._bkw(group))
         return kv_all
 
     def _kv_bwd(self, group, dkv_all, ykv, dykv):
-        """Weight gradient of the stacked kv_linear and the gradient flowing into the caption tokens."""
+        """Weight (and bias) gradient of the stacked kv_linear and the gradient flowing into the caption tokens."""
         o, st = self.ops, self.store
+        self._colsum(dkv_all, self._gb(group))
         self._wgrad(dkv_all, ykv, self._Gv(group))
         o.gemm(dkv_all, st.WT(group), dykv, epi=EPI_RESID, res=dykv)
 
@@ -147,18 +167,18 @@ class Engine:
         sv.xm = o.empty((M, D), BF16); sv.mean1 = o.empty((M,), F32); sv.rstd1 = o.empty((M,), F32)
         sv.x = self._ln_add(x, pend, sv.xm, sv.mean1, sv.rstd1, gamma=P[n + ".norm1.weight"], shift=sh_a, scale=sc_a, T=T)
         sv.qkv = o.empty((M, 3 * h), BF16)
-        o.gemm(sv.xm, st.W(n + ".attn.qkv.weight"), sv.qkv)
+        o.gemm(sv.xm, st.W(n + ".attn.qkv.weight"), sv.qkv, **self._bkw(n + ".attn.qkv.weight"))
         sv.rqk = o.empty((2, M), F32)  # ln_q and ln_k (utils.py:183-186) in one launch: adjacent slices of qkv
         o.rownorm_fwd(sv.qkv[:, :2 * h], sv.rqk, eps, nslice=2)
         sv.att = o.empty((M, h), BF16); sv.lse = o.empty((B, bs.heads, T), F32)
         o.attn_fwd(sv.qkv[:, :h], sv.qkv[:, h:2 * h], sv.qkv[:, 2 * h:], sv.att, sv.lse, B, bs.heads, T, T, hd)
         sv.ya = o.empty((M, D), BF16)
-        o.gemm(sv.att, st.W(n + ".attn.proj.weight"), sv.ya)
+        o.gemm(sv.att, st.W(n + ".attn.proj.weight"), sv.ya, **self._bkw(n + ".attn.proj.weight"))
         # ---- cross attention to the caption tokens (dit.py:237, utils.py:116-136)
         sv.xn2 = o.empty((M, D), BF16); sv.mean2 = o.empty((M,), F32); sv.rstd2 = o.empty((M,), F32)
         sv.x1 = self._ln_add(sv.x, (sv.ya, g_a), sv.xn2, sv.mean2, sv.rstd2, gamma=P[n + ".norm2.weight"], T=T)
         sv.qx = o.empty((M, D), BF16)
-        o.gemm(sv.xn2, st.W(n + ".cross_attn.q_linear.weight"), sv.qx)
+        o.gemm(sv.xn2, st.W(n + ".cross_attn.q_linear.weight"), sv.qx, **self._bkw(n + ".cross_attn.q_linear.weight"))
         sv.kv = kv  # this block's [B*L, 2D] column slice of the stage-wide K/V projection
         sv.rq2 = o.empty((M,), F32); sv.rk2 = o.empty((B * L,), F32)
         o.rownorm_fwd(sv.qx, sv.rq2, eps)
@@ -167,7 +187,7 @@ class Engine:
         sv.att2 = o.empty((M, D), BF16); sv.lse2 = o.empty((B, bs.xheads, T), F32)
         o.attn_fwd(sv.qx, sv.kv[:, :D], sv.kv[:, D:], sv.att2, sv.lse2, B, bs.xheads, T, L, hd)
         yx = o.empty((M, D), BF16)
-        o.gemm(sv.att2, st.W(n + ".cross_attn.proj.weight"), yx)
+        o.gemm(sv.att2, st.W(n + ".cross_attn.proj.weight"), yx, **self._bkw(n + ".cross_attn.proj.weight"))
         # ---- feed-forward (dit.py:238)
         sv.xm3 = o.empty((M, D), BF16); sv.mean3 = o.empty((M,), F32); sv.rstd3 = o.empty((M,), F32)
         sv.x2 = self._ln_add(sv.x1, (yx, None), sv.xm3, sv.mean3, sv.rstd3, gamma=P[n + ".norm3.weight"], shift=sh_m,
@@ -177,7 +197,7 @@ class Engine:
             sv.u = o.empty((M, 2 * f), BF16)
             sv.hact = o.empty((M, f), BF16)
             self._swiglu_fwd(n + ".mlp.w12", sv.xm3, sv.u, sv.hact)
-            o.gemm(sv.hact, st.W(n + ".mlp.w3.weight"), sv.ym)
+            o.gemm(sv.hact, st.W(n + ".mlp.w3.weight"), sv.ym, **self._bkw(n + ".mlp.w3.weight"))
             out, pend_out = sv.x2, (sv.ym, g_m)
         else:  # expert-choice MoE (dit.py:126-143): the combine kernel applies the gated residual itself
             E = cfg.num_experts
@@ -230,6 +250,7 @@ class Engine:
             dy = dy_in
         dxm = o.empty((M, D), BF16)
         if not bs.moe:
+            self._colsum(dy, self._gb(n + ".mlp.w3.weight"))
             du = o.empty((M, 2 * f), BF16)
             self._swiglu_bwd(n + ".mlp.w12", n + ".mlp.w3.weight", dy, sv.u, du)
             self._wgrad(dy, sv.hact, self._Gv(n + ".mlp.w3.weight"))
@@ -260,6 +281,7 @@ class Engine:
         # ---- cross attention branch (no gate, no modulation): dy = bf16(dx)
         if not fuse:
             o.gate_bwd(dx, dy, T=T)
+        self._colsum(dy, self._gb(n + ".cross_attn.proj.weight"))
         datt2 = o.empty((M, D), BF16)
         o.gemm(dy, st.WT(n + ".cross_attn.proj.weight"), datt2)
         self._wgrad(dy, sv.att2, self._Gv(n + ".cross_attn.proj.weight"))
@@ -269,6 +291,7 @@ class Engine:
                    bs.xheads, T, L, hd)
         o.rownorm_bwd(dqx, sv.qx, sv.rq2)
         o.rownorm_bwd(dkv[:, :D], sv.kv[:, :D], sv.rk2)
+        self._colsum(dqx, self._gb(n + ".cross_attn.q_linear.weight"))
         dxn2 = o.empty((M, D), BF16)
         o.gemm(dqx, st.WT(n + ".cross_attn.q_linear.weight"), dxn2)
         self._wgrad(dqx, sv.xn2, self._Gv(n + ".cross_attn.q_linear.weight"))
@@ -281,6 +304,7 @@ class Engine:
                      dgamma=self._gv(n + ".norm2.weight"))
             o.gate_bwd(dx, dy, y=sv.ya, gate=g_a, dgate=dg_a, T=T)
         # ---- self attention branch
+        self._colsum(dy, self._gb(n + ".attn.proj.weight"))
         datt = o.empty((M, h), BF16)
         o.gemm(dy, st.WT(n + ".attn.proj.weight"), datt)
         self._wgrad(dy, sv.att, self._Gv(n + ".attn.proj.weight"))
@@ -289,6 +313,7 @@ class Engine:
         o.attn_bwd(datt, sv.qkv[:, :h], sv.qkv[:, h:2 * h], sv.qkv[:, 2 * h:], sv.att, sv.lse, delta, dqkv[:, :h],
                    dqkv[:, h:2 * h], dqkv[:, 2 * h:], B, bs.heads, T, T, hd)
         o.rownorm_bwd(dqkv[:, :2 * h], sv.qkv[:, :2 * h], sv.rqk, nslice=2)
+        self._colsum(dqkv, self._gb(n + ".attn.qkv.weight"))
         dxm1 = o.empty((M, D), BF16)
         o.gemm(dqkv, st.WT(n + ".attn.qkv.weight"), dxm1)
         self._wgrad(dqkv, sv.xm, self._Gv(n + ".attn.qkv.weight"))
@@ -329,13 +354,14 @@ class Engine:
         s.yn1 = o.empty((R, D), BF16); s.m1 = o.empty((R,), F32); s.r1 = o.empty((R,), F32)
         o.ln_fwd(s.y0, s.yn1, s.m1, s.r1, gamma=P["y_emb_preprocess.norm1.weight"], T=L, eps=eps)
         s.qkv = o.empty((R, 3 * D), BF16)
-        o.gemm(s.yn1, st.W("y_emb_preprocess.attn.qkv.weight"), s.qkv)
+        o.gemm(s.yn1, st.W("y_emb_preprocess.attn.qkv.weight"), s.qkv, **self._bkw("y_emb_preprocess.attn.qkv.weight"))
         s.rqk = o.empty((2, R), F32)
         o.rownorm_fwd(s.qkv[:, :2 * D], s.rqk, eps, nslice=2)
         s.att = o.empty((R, D), BF16); s.lse = o.empty((B, H, L), F32)
         o.attn_fwd(s.qkv[:, :D], s.qkv[:, D:2 * D], s.qkv[:, 2 * D:], s.att, s.lse, B, H, L, L, hd)
         s.y1 = o.empty((R, D), F32)
-        o.gemm(s.att, st.W("y_emb_preprocess.attn.proj.weight"), s.y1, epi=EPI_RESID, res=s.y0)
+        o.gemm(s.att, st.W("y_emb_preprocess.attn.proj.weight"), s.y1, epi=EPI_RESID, res=s.y0,
+               **self._bkw("y_emb_preprocess.attn.proj.weight"))
         fp = cfg.prompt_ffn_dim
         s.yn2 = o.empty((R, D), BF16); s.m2 = o.empty((R,), F32); s.r2 = o.empty((R,), F32)
         o.ln_fwd(s.y1, s.yn2, s.m2, s.r2, gamma=P["y_emb_preprocess.norm2.weight"], T=L, eps=eps)
@@ -343,7 +369,8 @@ class Engine:
         s.hact = o.empty((R, fp), BF16)
         self._swiglu_fwd("y_emb_preprocess.mlp.w12", s.yn2, s.u, s.hact)
         s.y2 = o.empty((R, D), F32)
-        o.gemm(s.hact, st.W("y_emb_preprocess.mlp.w3.weight"), s.y2, epi=EPI_RESID, res=s.y1)
+        o.gemm(s.hact, st.W("y_emb_preprocess.mlp.w3.weight"), s.y2, epi=EPI_RESID, res=s.y1,
+               **self._bkw("y_emb_preprocess.mlp.w3.weight"))
         s.ybf = o.empty((R, D), BF16)
         o.cast_bf16(s.y2, s.ybf)
         # pooled caption -> Mlp (dit.py:484)
@@ -432,6 +459,7 @@ class Engine:
         fp = cfg.prompt_ffn_dim
         dyb = o.empty((R, D), BF16)
         o.gate_bwd(dy2, dyb, T=L)
+        self._colsum(dy2, self._gb("y_emb_preprocess.mlp.w3.weight"))
         du = o.empty((R, 2 * fp), BF16)
         self._swiglu_bwd("y_emb_preprocess.mlp.w12", "y_emb_preprocess.mlp.w3.weight", dyb, s.u, du)
         self._wgrad(dyb, s.hact, self._Gv("y_emb_preprocess.mlp.w3.weight"))
@@ -442,6 +470,7 @@ class Engine:
                  dgamma=self._gv("y_emb_preprocess.norm2.weight"))
         # ---- prompt block: self attention
         o.gate_bwd(dy2, dyb, T=L)
+        self._colsum(dy2, self._gb("y_emb_preprocess.attn.proj.weight"))
         datt = o.empty((R, D), BF16)
         o.gemm(dyb, st.WT("y_emb_preprocess.attn.proj.weight"), datt)
         self._wgrad(dyb, s.att, self._Gv("y_emb_preprocess.attn.proj.weight"))
@@ -449,6 +478,7 @@ class Engine:
         o.attn_bwd(datt, s.qkv[:, :D], s.qkv[:, D:2 * D], s.qkv[:, 2 * D:], s.att, s.lse, delta, dqkv[:, :D],
                    dqkv[:, D:2 * D], dqkv[:, 2 * D:], B, H, L, L, hd)
         o.rownorm_bwd(dqkv[:, :2 * D], s.qkv[:, :2 * D], s.rqk, nslice=2)
+        self._colsum(dqkv, self._gb("y_emb_preprocess.attn.qkv.weight"))
         o.gemm(dqkv, st.WT("y_emb_preprocess.attn.qkv.weight"), dyn)
         self._wgrad(dqkv, s.yn1, self._Gv("y_emb_preprocess.attn.qkv.weight"))
         o.ln_bwd(dyn, s.y0, s.m1, s.r1, gamma=P["y_emb_preprocess.norm1.weight"], T=L, dx=dy2, dx_mode=0,
@@ -488,7 +518,7 @@ class Engine:
                 y_n = o.empty((B * L, D), BF16); m = o.empty((B * L,), F32); r = o.empty((B * L,), F32)
                 o.ln_fwd(s.y2, y_n, m, r, gamma=P["patch_mixer_map_y.0.weight"], T=L, eps=eps)
                 pc.ymix = o.empty((B * L, Dm), BF16)
-                o.gemm(y_n, st.W("patch_mixer_map_y.1.weight"), pc.ymix)
+                o.gemm(y_n, st.W("patch_mixer_map_y.1.weight"), pc.ymix, **self._bkw("patch_mixer_map_y.1.weight"))
             else:
                 pc.ymix = s.ybf
             pc.kv_m = self._kv_fwd("kv.patch_mixer", pc.ymix, len(cfg.mixer_blocks), 2 * Dm)
@@ -547,12 +577,12 @@ class Engine:
                 c.xin_n = o.empty((B * T, D), BF16); c.m_xin = o.empty((B * T,), F32); c.r_xin = o.empty((B * T,), F32)
                 o.ln_fwd(x0, c.xin_n, c.m_xin, c.r_xin, gamma=P["patch_mixer_map_xin.0.weight"], T=T, eps=cfg.norm_eps)
                 xm = o.empty((B * T, Dm), F32)
-                o.gemm(c.xin_n, st.W("patch_mixer_map_xin.1.weight"), xm, epi=EPI_F32)
+                o.gemm(c.xin_n, st.W("patch_mixer_map_xin.1.weight"), xm, epi=EPI_F32, **self._bkw("patch_mixer_map_xin.1.weight"))
                 if prompt is None:
                     c.y_n = o.empty((B * L, D), BF16); c.m_y = o.empty((B * L,), F32); c.r_y = o.empty((B * L,), F32)
                     o.ln_fwd(s.y2, c.y_n, c.m_y, c.r_y, gamma=P["patch_mixer_map_y.0.weight"], T=L, eps=cfg.norm_eps)
                     c.ymix = o.empty((B * L, Dm), BF16)
-                    o.gemm(c.y_n, st.W("patch_mixer_map_y.1.weight"), c.ymix)
+                    o.gemm(c.y_n, st.W("patch_mixer_map_y.1.weight"), c.ymix, **self._bkw("patch_mixer_map_y.1.weight"))
             else:
                 xm, c.ymix = x0, s.ybf
             c.x0 = x0
@@ -578,7 +608,8 @@ class Engine:
             c.xm_out = self._ln_add(xm, pend, c.xk_n, c.m_xo, c.r_xo, gamma=P["patch_mixer_map_xout.0.weight"], T=Tk,
                                     src_rows=c.keep_rows)
             xb = o.empty((B * Tk, D), F32)
-            o.gemm(c.xk_n, st.W("patch_mixer_map_xout.1.weight"), xb, epi=EPI_F32)
+            o.gemm(c.xk_n, st.W("patch_mixer_map_xout.1.weight"), xb, epi=EPI_F32,
+                   **self._bkw("patch_mixer_map_xout.1.weight"))
             pend = None
         elif mask_ratio > 0:
             xm = self._materialize(xm, pend, T)
@@ -731,6 +762,7 @@ class Engine:
         if cfg.has_mixer_maps:
             dxb = o.empty((B * Tk, D), BF16)
             o.gate_bwd(dx, dxb, T=Tk)
+            self._colsum(dx, self._gb("patch_mixer_map_xout.1.weight"))
             self._wgrad(dxb, c.xk_n, self._Gv("patch_mixer_map_xout.1.weight"))
             dxk = o.empty((B * Tk, Dm), BF16)
             o.gemm(dxb, st.WT("patch_mixer_map_xout.1.weight"), dxk)
@@ -760,6 +792,7 @@ class Engine:
                 # caption map: y_mixer = Linear(LN(y))
                 dymb = o.empty((B * L, Dm), BF16)
                 o.gate_bwd(dymix, dymb, T=L)
+                self._colsum(dymix, self._gb("patch_mixer_map_y.1.weight"))
                 self._wgrad(dymb, c.y_n, self._Gv("patch_mixer_map_y.1.weight"))
                 dyn = o.empty((B * L, D), BF16)
                 o.gemm(dymb, st.WT("patch_mixer_map_y.1.weight"), dyn)
@@ -768,6 +801,7 @@ class Engine:
                 # token map: x_mixer = Linear(LN(x0))
                 dxmb = o.empty((B * T, Dm), BF16)
                 o.gate_bwd(dxm, dxmb, T=T)
+                self._colsum(dxm, self._gb("patch_mixer_map_xin.1.weight"))
                 self._wgrad(dxmb, c.xin_n, self._Gv("patch_mixer_map_xin.1.weight"))
                 dxn = o.empty((B * T, D), BF16)
                 o.gemm(dxmb, st.WT("patch_mixer_map_xin.1.weight"), dxn)

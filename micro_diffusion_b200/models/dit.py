@@ -95,7 +95,9 @@ class DiT(nn.Module):
                              patch_mixer_mlp_ratio=patch_mixer_mlp_ratio, use_bias=use_bias, num_experts=num_experts,
                              expert_capacity=expert_capacity, experts_every_n=experts_every_n)
         if not use_patch_mixer:
-            raise NotImplementedError("use_patch_mixer=False is not on the MicroDiT path (dit.py:657,698)")
+            raise NotImplementedError("use_patch_mixer=False is not supported: the reference cannot build it either (its "
+                                      "initialize_weights reads self.patch_mixer, which only exists with the mixer, "
+                                      "dit.py:612)")
         # attributes the reference exposes (dit.py:303-309) and LatentDiffusion / callbacks read
         self.input_size, self.in_channels, self.out_channels = input_size, in_channels, in_channels
         self.patch_size, self.head_dim, self.pos_interp_scale = patch_size, head_dim, pos_interp_scale

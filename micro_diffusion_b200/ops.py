@@ -74,6 +74,7 @@ _PROTOS = {
     "md_mean_tokens_bwd": [_P, _P, _I64, _I64, _I64, _P],
     "md_cast_f32_bf16": [_P, _P, _I64, _I, _P],
     "md_colsum": [_P, _I, _I64, _P, _I64, _I64, _P],
+    "md_colsum_interleaved": [_P, _I, _I64, _P, _I64, _I64, _I64, _P],
     "md_cast_transpose": [_P, _P, _P, _I64, _I64, _I64, _I64, _I, _P],
     "md_cast_transpose_multi": [_P, _P, _P, _P, _I64, _I64, _I, _P],
     "md_set_deterministic": [_P, _I64],
@@ -269,6 +270,8 @@ class CudaOps:
         a.ldc2 = a.strideC2 = 0
         if epi == EPI_SWIGLU:
             assert C2 is not None and C2.dtype == torch.bfloat16 and C2.shape[-1] == N // 2 and C2.stride(-1) == 1
+            # the bias is the natural-order [b1 | b2] vector; the epilogue maps it onto the interleaved columns
+            assert bias is None or (bias.dtype == torch.float32 and bias.shape[-1] == N and bias.stride(-1) == 1)
             a.ldc2 = C2.stride(-2)
             a.strideC2 = C2.stride(0) if C2.dim() == 3 else 0
         elif C2 is not None:
@@ -501,6 +504,13 @@ class CudaOps:
     def colsum(self, x, out):
         rows, N = x.shape
         self._call("md_colsum", x.data_ptr(), int(x.dtype == torch.bfloat16), x.stride(0), out.data_ptr(), rows, N)
+
+    def colsum_interleaved(self, x, out, half):
+        """out(f32 [2 half]) += column sums of x [rows, 2 half] (32-interleaved w1 | w2 columns), in [b1 | b2] order."""
+        rows, N = x.shape
+        assert N == 2 * half and out.numel() == N and out.dtype == torch.float32
+        self._call("md_colsum_interleaved", x.data_ptr(), int(x.dtype == torch.bfloat16), x.stride(0), out.data_ptr(), rows,
+                   N, half)
 
     def cast_transpose(self, w, wb, wbt, interleave_half=0):
         if w.dim() == 2:

@@ -60,9 +60,21 @@ class ParamLayout:
         # utils.py:118): stacking their weights turns 28 (+6) medium GEMMs per direction into one large one.
         kv_m = [s for s in specs if s[0].startswith("patch_mixer.") and s[0].endswith("cross_attn.kv_linear.weight")]
         kv_b = [s for s in specs if s[0].startswith("blocks.") and s[0].endswith("cross_attn.kv_linear.weight")]
-        special = {s[0] for s in ada_w + ada_b + kv_m + kv_b}
-        rest = [s for s in specs if s[0] not in special]
-        self.order: List[Tuple[str, Tuple[int, ...]]] = ada_w + ada_b + kv_m + kv_b + rest
+        # use_bias=True: the kv_linear biases of a stage follow its weight stack as one [nblk * 2D] vector (the bias of the
+        # stacked GEMM), in block order
+        kvb_m = [s for s in specs if s[0].startswith("patch_mixer.") and s[0].endswith("cross_attn.kv_linear.bias")]
+        kvb_b = [s for s in specs if s[0].startswith("blocks.") and s[0].endswith("cross_attn.kv_linear.bias")]
+        special = {s[0] for s in ada_w + ada_b + kv_m + kv_b + kvb_m + kvb_b}
+        shapes = dict(specs)
+        rest = []
+        for name, shape in specs:
+            if name in special or name.endswith("mlp.w1.bias"):
+                continue  # w1.bias is placed after w2.weight below, so that the two weights stay adjacent (the w12 stack)
+            rest.append((name, shape))
+            b1 = name[: -len("w2.weight")] + "w1.bias"
+            if name.endswith("mlp.w2.weight") and b1 in shapes:
+                rest.append((b1, shapes[b1]))  # a SwiGLU's biases as one [b1 | b2] vector after the w1 | w2 weights
+        self.order: List[Tuple[str, Tuple[int, ...]]] = ada_w + ada_b + kv_m + kvb_m + kv_b + kvb_b + rest
         self.reference_order = [s[0] for s in specs]
         self.slots: Dict[str, Tuple[int, Tuple[int, ...]]] = {}
         # The flat buffer is exchanged in a few contiguous ranges (train_step.GradReducer): "back" = the stacked backbone
@@ -142,6 +154,21 @@ class ParamLayout:
                 need_t = name != "y_embedder.y_proj.fc1.weight"  # input is data: no dgrad
                 self.groups[name] = MatGroup(name, o, 1, shape[0], shape[1], need_t=need_t)
 
+        # use_bias=True: the fp32 bias vector of each stacked GEMM, group name -> (offset, length).  A w12 stack's is
+        # [b1 | b2] in the parameters' own order; a kv.* stack's is every block's [2D] kv_linear bias in block order.
+        self.bias: Dict[str, Tuple[int, int]] = {}
+        for gname, lst in (("kv.patch_mixer", kvb_m), ("kv.blocks", kvb_b)):
+            if lst:
+                o0, n = self.slots[lst[0][0]][0], sum(s[1][0] for s in lst)
+                assert self.slots[lst[-1][0]][0] + lst[-1][1][0] - o0 == n, "kv bias stack must be contiguous"
+                self.bias[gname] = (o0, n)
+        for gname, g in self.groups.items():
+            pre = gname[: -len("w12")]
+            if gname.endswith(".w12") and pre + "w1.bias" in self.slots:
+                o1, f = self.slots[pre + "w1.bias"][0], g.rows // 2
+                assert self.slots[pre + "w2.bias"][0] == o1 + f, "b1 / b2 must be adjacent"
+                self.bias[gname] = (o1, 2 * f)
+
 
 class ParamStore:
     """Device buffers for one DiT: fp32 master + grad, bf16 copies, views."""
@@ -194,6 +221,25 @@ class ParamStore:
     def G(self, name: str) -> torch.Tensor:
         """fp32 gradient view of a group in its own layout."""
         return self._gview(self.grad, self.layout.groups[name])
+
+    def _bias_slice(self, buf, key: str):
+        hit = self.layout.bias.get(key)
+        if hit is not None:
+            return buf[hit[0]: hit[0] + hit[1]]
+        if key.endswith(".weight"):
+            hit = self.layout.slots.get(key[: -len("weight")] + "bias")
+            if hit is not None:
+                return buf[hit[0]: hit[0] + hit[1][0]]
+        return None
+
+    def bias(self, key: str):
+        """fp32 bias of a GEMM group (a w12 or kv.* stack) or of a single Linear given by its weight name; None when the
+        layer has no bias."""
+        return self._bias_slice(self.flat, key)
+
+    def gbias(self, key: str):
+        """Gradient view matching bias(key)."""
+        return self._bias_slice(self.grad, key)
 
     def is_back(self, offset: int) -> bool:
         """True for tensors of the "back" exchange ranges (backbone blocks, final layer, stacked backbone K/V)."""

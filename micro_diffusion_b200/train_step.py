@@ -105,11 +105,10 @@ class GradReducer:
         first = min(off for name, (off, _) in lay.slots.items()
                     if (name.startswith("blocks.") or name.startswith("final_layer."))
                     and not name.endswith("adaLN_modulation.1.weight") and not name.endswith("adaLN_modulation.1.bias")
-                    and not name.endswith("cross_attn.kv_linear.weight"))
+                    and not name.endswith("cross_attn.kv_linear.weight") and not name.endswith("cross_attn.kv_linear.bias"))
         self.early = [(first, n)]
-        if "kv.blocks" in lay.groups:
-            g = lay.groups["kv.blocks"]
-            self.early.append((g.offset, g.offset + g.numel))
+        if lay.kv_back is not None:  # part 2: the stacked backbone K/V projection, its bias stack included
+            self.early.append(lay.kv_back)
         # late = the complement
         cuts = sorted(self.early)
         self.late, pos = [], 0
