@@ -338,6 +338,17 @@ MD_API int md_sumsq(const float* x, float* sumsq, int64_t n, void* stream);
 MD_API int md_adamw(float* p, const float* g, float* m, float* v, const float* sumsq, float clip, float lr,
                     float beta1, float beta2, float eps, float wd, int64_t step, int32_t* nonfinite, int64_t n,
                     void* stream);
+/* md_adamw plus an exponential moving average of the weights in the same pass: p / m / v get the same update as
+ * md_adamw (bit-identical: one shared device function), then ema = smoothing * ema + (1 - smoothing) * p_new from the
+ * register holding p_new -- 8 more bytes per parameter, p is not read twice.  smoothing in [0, 1].  A non-finite
+ * sumsq[0] writes nothing (p, m, v and ema) and sets *nonfinite.  All five pointers 16-byte aligned (float4 body,
+ * scalar tail).  Element-wise, no reduction: bit-reproducible with or without deterministic mode. */
+MD_API int md_adamw_ema(float* p, const float* g, float* m, float* v, const float* sumsq, float clip, float lr,
+                        float beta1, float beta2, float eps, float wd, int64_t step, float* ema, float smoothing,
+                        int32_t* nonfinite, int64_t n, void* stream);
+/* Exchange a[0, n) and b[0, n) in place (swapping EMA and training weights without a full-size temporary).  a == b and
+ * any other overlap of the two ranges are rejected.  Element-wise, no reduction: deterministic mode needs nothing. */
+MD_API int md_swap_f32(float* a, float* b, int64_t n, void* stream);
 
 #ifdef __cplusplus
 }

@@ -331,19 +331,35 @@ __global__ void sumsq_kernel(const float* __restrict__ x, float* __restrict__ ou
   }
 }
 
+// One parameter's AdamW update, in place.  md_adamw and md_adamw_ema both run exactly this, so their p / m / v agree
+// bit for bit.  The moment updates spell out their FMA (m = b1 m + (1 - b1) gg, v = b2 v + (1 - b2) gg^2), which the
+// compiler would otherwise contract differently at different call sites.
+__device__ __forceinline__ void adamw_elem(float& p, float g, float& m, float& v, float gs, float lr, float b1, float b2,
+                                           float eps, float wd, float bc1, float bc2) {
+  const float gg = g * gs;
+  p *= 1.f - lr * wd;
+  m = __fmaf_rn(1.f - b1, gg, b1 * m);
+  v = __fmaf_rn(gg, (1.f - b2) * gg, b2 * v);
+  const float denom = sqrtf(v) / sqrtf(bc2) + eps;
+  p -= (lr / bc1) * m / denom;
+}
+
+// kEma: also ema = s * ema + (1 - s) * p_new, from the register that holds p_new (8 more bytes per parameter).
+template <bool kEma>
 __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                              float* __restrict__ v, const float* __restrict__ sumsq, float clip, float lr, float b1,
                              float b2, float eps, float wd, float bc1, float bc2, int* __restrict__ nonfinite,
-                             long long n) {
+                             long long n, float* __restrict__ ema, float s) {
   float gs = 1.f;
   if (sumsq != nullptr) {
     const float ss = sumsq[0];
-    if (!isfinite(ss)) {  // a NaN / Inf gradient anywhere: leave weights and moments untouched (NaNCatcher, callbacks.py:47-64)
+    if (!isfinite(ss)) {  // a NaN / Inf gradient anywhere: leave weights, moments and EMA untouched (NaNCatcher, callbacks.py:47-64)
       if (nonfinite != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *nonfinite = 1;
       return;
     }
     if (clip > 0.f) gs = fminf(1.f, clip / (sqrtf(ss) + 1e-6f));
   }
+  const float s1 = 1.f - s;
   const long long nv = n >> 2;
   for (long long i = 1LL * blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += 1LL * gridDim.x * blockDim.x) {
     float4 pv = *reinterpret_cast<float4*>(p + 4 * i);
@@ -355,26 +371,53 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
     float* mp = reinterpret_cast<float*>(&mv);
     float* vp = reinterpret_cast<float*>(&vv);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float gg = gp[e] * gs;
-      pp[e] *= 1.f - lr * wd;
-      mp[e] = b1 * mp[e] + (1.f - b1) * gg;
-      vp[e] = b2 * vp[e] + (1.f - b2) * gg * gg;
-      const float denom = sqrtf(vp[e]) / sqrtf(bc2) + eps;
-      pp[e] -= (lr / bc1) * mp[e] / denom;
-    }
+    for (int e = 0; e < 4; ++e) adamw_elem(pp[e], gp[e], mp[e], vp[e], gs, lr, b1, b2, eps, wd, bc1, bc2);
     *reinterpret_cast<float4*>(p + 4 * i) = pv;
     *reinterpret_cast<float4*>(m + 4 * i) = mv;
     *reinterpret_cast<float4*>(v + 4 * i) = vv;
+    if (kEma) {
+      float4 ev = *reinterpret_cast<float4*>(ema + 4 * i);
+      ev.x = s * ev.x + s1 * pv.x;
+      ev.y = s * ev.y + s1 * pv.y;
+      ev.z = s * ev.z + s1 * pv.z;
+      ev.w = s * ev.w + s1 * pv.w;
+      *reinterpret_cast<float4*>(ema + 4 * i) = ev;
+    }
   }
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
     const long long i = (nv << 2) + threadIdx.x;
-    const float gg = g[i] * gs;
-    float pp = p[i] * (1.f - lr * wd);
-    const float mm = b1 * m[i] + (1.f - b1) * gg;
-    const float vv = b2 * v[i] + (1.f - b2) * gg * gg;
-    pp -= (lr / bc1) * mm / (sqrtf(vv) / sqrtf(bc2) + eps);
+    float pp = p[i], mm = m[i], vv = v[i];
+    adamw_elem(pp, g[i], mm, vv, gs, lr, b1, b2, eps, wd, bc1, bc2);
     p[i] = pp; m[i] = mm; v[i] = vv;
+    if (kEma) ema[i] = s * ema[i] + s1 * pp;
+  }
+}
+
+// a <-> b, element by element (kVec: both 16-byte aligned, float4 body + scalar tail)
+template <bool kVec>
+__global__ void swap_f32_kernel(float* __restrict__ a, float* __restrict__ b, long long n) {
+  const long long stride = 1LL * gridDim.x * blockDim.x;
+  long long i = 1LL * blockIdx.x * blockDim.x + threadIdx.x;
+  if (kVec) {
+    const long long nv = n >> 2;
+    for (; i < nv; i += stride) {
+      const float4 x = *reinterpret_cast<const float4*>(a + 4 * i);
+      const float4 y = *reinterpret_cast<const float4*>(b + 4 * i);
+      *reinterpret_cast<float4*>(a + 4 * i) = y;
+      *reinterpret_cast<float4*>(b + 4 * i) = x;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+      const long long j = (nv << 2) + threadIdx.x;
+      const float x = a[j];
+      a[j] = b[j];
+      b[j] = x;
+    }
+  } else {
+    for (; i < n; i += stride) {
+      const float x = a[i];
+      a[i] = b[i];
+      b[i] = x;
+    }
   }
 }
 
@@ -522,7 +565,34 @@ extern "C" int md_adamw(float* p, const float* g, float* m, float* v, const floa
   if (n == 0) return 0;
   if (!p || !g || !m || !v || step < 1) return md_set_error(MD_ERR_INVALID, "md_adamw: null pointer or step < 1");
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-  adamw_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(p, g, m, v, sumsq, clip, lr, beta1, beta2, eps, wd,
-                                                                 bc1, bc2, nonfinite, n);
+  adamw_kernel<false><<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(p, g, m, v, sumsq, clip, lr, beta1, beta2, eps,
+                                                                        wd, bc1, bc2, nonfinite, n, nullptr, 0.f);
   return check_launch("md_adamw");
+}
+extern "C" int md_adamw_ema(float* p, const float* g, float* m, float* v, const float* sumsq, float clip, float lr,
+                            float beta1, float beta2, float eps, float wd, int64_t step, float* ema, float smoothing,
+                            int32_t* nonfinite, int64_t n, void* stream) {
+  if (n == 0) return 0;
+  if (!p || !g || !m || !v || !ema || step < 1)
+    return md_set_error(MD_ERR_INVALID, "md_adamw_ema: null pointer or step < 1");
+  if (!(smoothing >= 0.f && smoothing <= 1.f))
+    return md_set_error(MD_ERR_INVALID, "md_adamw_ema: smoothing must lie in [0, 1]");
+  if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+       reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(ema)) & 15)
+    return md_set_error(MD_ERR_INVALID, "md_adamw_ema: p, g, m, v and ema must be 16-byte aligned");
+  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
+  adamw_kernel<true><<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(p, g, m, v, sumsq, clip, lr, beta1, beta2, eps,
+                                                                       wd, bc1, bc2, nonfinite, n, ema, smoothing);
+  return check_launch("md_adamw_ema");
+}
+extern "C" int md_swap_f32(float* a, float* b, int64_t n, void* stream) {
+  if (n == 0) return 0;
+  if (!a || !b || n < 0) return md_set_error(MD_ERR_INVALID, "md_swap_f32: null pointer or n < 0");
+  if (a == b) return md_set_error(MD_ERR_INVALID, "md_swap_f32: a and b are the same range");
+  if (a < b + n && b < a + n) return md_set_error(MD_ERR_INVALID, "md_swap_f32: the two ranges overlap");
+  if (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0)
+    swap_f32_kernel<true><<<grid_for(n / 4 + 1, 256), 256, 0, ST(stream)>>>(a, b, n);
+  else
+    swap_f32_kernel<false><<<grid_for(n, 256), 256, 0, ST(stream)>>>(a, b, n);
+  return check_launch("md_swap_f32");
 }

@@ -80,6 +80,8 @@ _PROTOS = {
     "md_set_deterministic": [_P, _I64],
     "md_sumsq": [_P, _P, _I64, _P],
     "md_adamw": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _F, _F, _I64, _P, _I64, _P],
+    "md_adamw_ema": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _F, _F, _I64, _P, _F, _P, _I64, _P],
+    "md_swap_f32": [_P, _P, _I64, _P],
 }
 
 _TAKES_PREC = frozenset(['md_ln_fwd', 'md_ln_bwd', 'md_rownorm_fwd', 'md_rownorm_bwd', 'md_gate_bwd', 'md_swiglu_fwd', 'md_swiglu_bwd', 'md_act_fwd', 'md_act_bwd', 'md_gelu_tanh_f32_fwd', 'md_moe_gate_fwd', 'md_moe_gather', 'md_moe_combine_fwd', 'md_moe_combine_bwd', 'md_moe_dx_bwd', 'md_moe_gate_wgrad', 'md_cond_prepare', 'md_edm_prepare', 'md_patchify', 'md_timestep_embed', 'md_edm_loss_bwd', 'md_unpatchify_bwd', 'md_patchify_bwd', 'md_timestep_embed_bwd', 'md_mean_tokens_fwd', 'md_cast_f32_bf16', 'md_cast_transpose', 'md_cast_transpose_multi'])
@@ -531,3 +533,14 @@ class CudaOps:
     def adamw(self, p, g, m, v, sumsq, clip, lr, beta1, beta2, eps, wd, step, nonfinite=None):
         self._call("md_adamw", p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), _ptr(sumsq), clip, lr, beta1,
                    beta2, eps, wd, step, _ptr(nonfinite), p.numel())
+
+    def adamw_ema(self, p, g, m, v, sumsq, clip, lr, beta1, beta2, eps, wd, step, ema, smoothing, nonfinite=None):
+        """adamw(...) and, in the same pass, ema = smoothing * ema + (1 - smoothing) * p_new."""
+        assert ema.numel() == p.numel() and ema.dtype == torch.float32
+        self._call("md_adamw_ema", p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), _ptr(sumsq), clip, lr, beta1,
+                   beta2, eps, wd, step, ema.data_ptr(), smoothing, _ptr(nonfinite), p.numel())
+
+    def swap(self, a, b):
+        """Exchange the contents of two fp32 buffers of the same size in place (md_swap_f32; they may not overlap)."""
+        assert a.numel() == b.numel() and a.dtype == b.dtype == torch.float32 and a.is_contiguous() and b.is_contiguous()
+        self._call("md_swap_f32", a.data_ptr(), b.data_ptr(), a.numel())

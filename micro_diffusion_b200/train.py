@@ -6,7 +6,7 @@
 The file format and the keys are the reference's (configs/res_*.yaml; consumed by train.py:14-126): `model` (the
 `create_latent_diffusion` kwargs), `dataset` (+ `dataset.train`: the latents dataloader kwargs), `optimizer`
 (torch.optim.AdamW kwargs), `scheduler` (Composer's CosineAnnealingWithWarmup / Constant / ConstantWithWarmup), `algorithms.gradient_clipping`,
-`trainer` (max_duration, save/load options, device_train_microbatch_size), `seed`.  `${key}` / `${a.b}` interpolation
+`algorithms.ema` (an EMA of the weights, ema.FlatEMA; the override `algorithms.ema=null` turns it off), `trainer` (max_duration, save/load options, device_train_microbatch_size), `seed`.  `${key}` / `${a.b}` interpolation
 and `a.b=value` command-line overrides follow OmegaConf's surface for the subset the configs use.  What the hot path
 does not cover is accepted and ignored with a note: loggers, the image-monitor callback,
 `misc.compile`, `fsdp_config` (weights are replicated, gradients all-reduced -- train_step.GradReducer), and
@@ -111,7 +111,39 @@ def trainer_kwargs(cfg: dict) -> Dict[str, Any]:
         load_strict_model_weights=bool(tr.get("load_strict_model_weights", True)),
         load_ignore_keys=tuple(tr.get("load_ignore_keys") or ()),
         save_num_checkpoints_to_keep=tr.get("save_num_checkpoints_to_keep"),
+        **ema_kwargs(cfg),
     )
+
+
+_EMA_FIELDS = ("_target_", "half_life", "smoothing", "update_interval", "ema_start")
+
+
+def ema_kwargs(cfg: dict) -> Dict[str, Any]:
+    """`algorithms.ema` (configs/res_512_pretrain.yaml:3-9, any `_target_` ending in `.EMA`) as Trainer arguments;
+    {} when the section is absent or null (`algorithms.ema=null` turns a config's EMA off).  What the trainer cannot
+    honour raises: both or neither of half_life / smoothing, units other than batches, unknown fields."""
+    ema = (cfg.get("algorithms") or {}).get("ema")
+    if not ema:
+        return {}
+    target = str(ema.get("_target_", ""))
+    if not target.endswith(".EMA"):
+        raise ValueError(f"algorithms.ema: expected an EMA algorithm (_target_ ending in .EMA), got {target!r}")
+    unknown = sorted(set(ema) - set(_EMA_FIELDS))
+    if unknown:
+        raise ValueError(f"algorithms.ema: unsupported fields {unknown}")
+    hl, sm = ema.get("half_life"), ema.get("smoothing")
+    if (hl is None) == (sm is None):
+        raise ValueError("algorithms.ema: set exactly one of half_life and smoothing")
+    from .trainer import parse_batches
+    interval, start = ema.get("update_interval") or "1ba", ema.get("ema_start") or "0ba"
+    for name, val in (("half_life", hl), ("update_interval", interval), ("ema_start", start)):
+        if val is not None:
+            try:
+                parse_batches(val)
+            except ValueError as e:
+                raise ValueError(f"algorithms.ema.{name}: {e}") from None
+    return dict(ema_smoothing=None if sm is None else float(sm), ema_half_life=hl, ema_update_interval=interval,
+                ema_start=start)
 
 
 def build(cfg: dict, device, rank: int = 0, world: int = 1, model=None):
@@ -173,6 +205,10 @@ def main(argv: Optional[List[str]] = None):
         for note in ignored_sections(cfg):
             print(f"[micro_diffusion_b200.train] ignoring {note}")
     _, _, trainer = build(cfg, device, rank, world)
+    if rank == 0 and trainer.ema is not None:
+        e = trainer.ema
+        print(f"[micro_diffusion_b200.train] EMA of the weights (smoothing {e.smoothing:.6g} every {e.update_interval} "
+              f"batches) starts after batch {e.ema_start}")
     loss = trainer.fit()
     if world > 1:
         dist.destroy_process_group()

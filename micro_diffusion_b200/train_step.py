@@ -35,9 +35,11 @@ class FlatAdamW:
         self.t = 0
 
     @torch.no_grad()
-    def step(self, lr: Optional[float] = None, reducer: Optional["GradReducer"] = None):
+    def step(self, lr: Optional[float] = None, reducer: Optional["GradReducer"] = None, ema=None):
         """`reducer` with `shard` set: the gradient is only valid on this rank's shares (reduce-scatter), so clip + AdamW
-        run on those segments -- the squared norm is summed over ranks -- and the updated parameters are all-gathered."""
+        run on those segments -- the squared norm is summed over ranks -- and the updated parameters are all-gathered.
+        `ema` (ema.FlatEMA): when an EMA update is due at this step, md_adamw_ema replaces md_adamw on the same segments;
+        otherwise the launches are those of a step without EMA."""
         eng = self.dit.engine
         st, o = eng.store, eng.ops
         self.t += 1
@@ -55,10 +57,18 @@ class FlatAdamW:
             # norm can differ in the last bit from rank to rank -- and with it the clip factor and every updated weight.
             # Rank 0's value is the value: replicas stay bit-identical (there is no parameter broadcast to repair drift).
             dist.broadcast(self.sumsq, src=0, group=reducer.group)
+        fused = ema is not None and ema.due(self.t)
         for a, b in segs:
-            o.adamw(st.flat[a:b], st.grad[a:b], self.m[a:b], self.v[a:b], self.sumsq, float(self.clip or 0.0),
-                    float(lr if lr is not None else self.lr), self.betas[0], self.betas[1], self.eps, self.wd, self.t,
-                    nonfinite=self.nonfinite)
+            if fused:
+                o.adamw_ema(st.flat[a:b], st.grad[a:b], self.m[a:b], self.v[a:b], self.sumsq, float(self.clip or 0.0),
+                            float(lr if lr is not None else self.lr), self.betas[0], self.betas[1], self.eps, self.wd,
+                            self.t, ema.ema[a:b], ema.smoothing, nonfinite=self.nonfinite)
+            else:
+                o.adamw(st.flat[a:b], st.grad[a:b], self.m[a:b], self.v[a:b], self.sumsq, float(self.clip or 0.0),
+                        float(lr if lr is not None else self.lr), self.betas[0], self.betas[1], self.eps, self.wd, self.t,
+                        nonfinite=self.nonfinite)
+        if ema is not None:
+            ema.after_step(self.t, segs, reducer if sharded else None)  # the start copy reads this rank's new weights
         if sharded:
             reducer.gather_params(st)
             self.sharded_by = reducer
@@ -215,9 +225,9 @@ class GradReducer:
 
 
 def train_step(model, batch: Dict[str, torch.Tensor], optimizer: FlatAdamW, reducer: Optional[GradReducer] = None,
-               microbatch: int = 256, lr: Optional[float] = None) -> torch.Tensor:
+               microbatch: int = 256, lr: Optional[float] = None, ema=None) -> torch.Tensor:
     """One optimisation step over `batch` (this rank's share of the global batch) at learning rate `lr` (default: the
-    optimizer's base rate): returns the mean loss (device)."""
+    optimizer's base rate), with the weight EMA `ema` (ema.FlatEMA) if given: returns the mean loss (device)."""
     B = batch["image_latents"].shape[0]
     total = None
     eng = model.dit.engine
@@ -233,6 +243,6 @@ def train_step(model, batch: Dict[str, torch.Tensor], optimizer: FlatAdamW, redu
         total = loss.detach() * (n / B) if total is None else total + loss.detach() * (n / B)
     if reducer is not None:
         reducer.reduce()
-    optimizer.step(lr, reducer)
+    optimizer.step(lr, reducer, ema)
     optimizer.zero_grad()
     return total

@@ -24,6 +24,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Sequence
 
 import torch
 
+from .ema import FlatEMA
 from .train_step import FlatAdamW, GradReducer, train_step
 
 
@@ -94,15 +95,22 @@ def _rng_state(device) -> dict:
     return st
 
 
+_EMA_KEYS = ("ema_weights", "started", "smoothing", "update_interval", "ema_start")
+
+
 def save_checkpoint(path: str, model, optimizer: Optional[FlatAdamW], batch: int, rank: int = 0, loader=None,
-                    world: int = 1, keep: Optional[int] = None) -> None:
+                    world: int = 1, keep: Optional[int] = None, ema: Optional[FlatEMA] = None) -> None:
     """Rank 0 writes; parameters are replicated so there is nothing to gather except the per-rank RNG states
     (every rank calls this).  `loader.state_dict()` (epoch, batch in epoch) and the RNG states are what Composer's
     checkpoint restores so that a resumed run continues the sample / noise / mask streams instead of replaying them.
-    `keep` = Composer's save_num_checkpoints_to_keep (configs/res_256_pretrain.yaml:112): older ba*.pt are removed."""
+    `keep` = Composer's save_num_checkpoints_to_keep (configs/res_256_pretrain.yaml:112): older ba*.pt are removed.
+    `ema`: its weights go to state["algorithms"]["EMA"]["ema_weights"] ("dit.<param>" keys, empty before the EMA has
+    started); state["model"] stays the training weights."""
     rng = [_rng_state(model.dit.store.device)]
     if optimizer is not None:
         optimizer.gather_state()  # sharded optimizer: every rank takes part in completing the moments
+    if ema is not None:
+        ema.gather_state()
     if world > 1:
         import torch.distributed as dist
         gathered = [None] * world
@@ -120,6 +128,10 @@ def save_checkpoint(path: str, model, optimizer: Optional[FlatAdamW], batch: int
         state["optimizers"] = {"FlatAdamW": {"exp_avg": optimizer.m.cpu(), "exp_avg_sq": optimizer.v.cpu(),
                                              "step": optimizer.t,
                                              "layout": list(model.dit.store.layout.slots.keys())}}
+    if ema is not None:
+        state["algorithms"] = {"EMA": {"ema_weights": ema.state_tensors() if ema.started else {},
+                                       "started": bool(ema.started), "smoothing": ema.smoothing,
+                                       "update_interval": ema.update_interval, "ema_start": ema.ema_start}}
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     tmp = path + ".tmp"
     torch.save({"state": state, "rng": rng}, tmp)
@@ -134,9 +146,11 @@ def save_checkpoint(path: str, model, optimizer: Optional[FlatAdamW], batch: int
 
 def load_checkpoint(path: str, model, optimizer: Optional[FlatAdamW] = None, load_weights_only: bool = False,
                     load_strict_model_weights: bool = True, load_ignore_keys: Sequence[str] = (), loader=None,
-                    rank: int = 0) -> int:
+                    rank: int = 0, ema: Optional[FlatEMA] = None) -> int:
     """Returns the batch count to resume from (0 with `load_weights_only`).  A full load also restores this rank's
-    RNG state and the loader position saved by `save_checkpoint` (dropped like any other entry by `load_ignore_keys`)."""
+    RNG state, the loader position and the EMA saved by `save_checkpoint` (dropped like any other entry by
+    `load_ignore_keys`).  An EMA entry that is missing, incomplete (e.g. partly dropped) or not started leaves `ema`
+    unstarted: it then starts again on its own schedule.  The schedule itself (smoothing, interval, start) is `ema`'s."""
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     if load_ignore_keys:
         _drop_ignored(ckpt, list(load_ignore_keys))
@@ -155,6 +169,11 @@ def load_checkpoint(path: str, model, optimizer: Optional[FlatAdamW] = None, loa
         optimizer.m.copy_(opt["exp_avg"])
         optimizer.v.copy_(opt["exp_avg_sq"])
         optimizer.t = int(opt["step"])
+    if ema is not None:
+        ema.started = False
+        entry = _ema_entry(ckpt)
+        if entry is not None:
+            ema.load_tensors(entry["ema_weights"])
     ds_state = ckpt["state"].get("dataset_state")
     if loader is not None and ds_state is not None and hasattr(loader, "load_state_dict"):
         loader.load_state_dict(ds_state)
@@ -164,6 +183,33 @@ def load_checkpoint(path: str, model, optimizer: Optional[FlatAdamW] = None, loa
         if "cuda" in rng[rank] and torch.device(model.dit.store.device).type == "cuda":
             torch.cuda.set_rng_state(rng[rank]["cuda"], model.dit.store.device)
     return int(ckpt["state"].get("timestamp", {}).get("batch", 0))
+
+
+def _ema_entry(ckpt: dict) -> Optional[dict]:
+    """state["algorithms"]["EMA"] if it holds started EMA weights and every schedule field, else None."""
+    entry = (ckpt["state"].get("algorithms") or {}).get("EMA")
+    if not isinstance(entry, dict) or any(k not in entry for k in _EMA_KEYS):
+        return None
+    if not entry["started"] or not isinstance(entry["ema_weights"], dict) or not entry["ema_weights"]:
+        return None
+    return entry
+
+
+def ema_state_dict(path: str) -> dict:
+    """A DiT state_dict of the checkpoint's EMA weights plus its buffers (pos_embed, ...), for
+    `model.dit.load_state_dict(ema_state_dict(path))` -- sampling from the EMA.  Raises if the checkpoint holds no
+    complete EMA entry."""
+    ckpt = torch.load(path, map_location="cpu", weights_only=False)
+    entry = _ema_entry(ckpt)
+    if entry is None:
+        raise ValueError(f"{path} holds no (complete) EMA weights")
+    sd = {k[len("dit."):]: v for k, v in ckpt["state"]["model"].items() if k.startswith("dit.")}
+    for k, v in entry["ema_weights"].items():
+        name = k[len("dit."):]
+        if name not in sd:
+            raise ValueError(f"{path}: EMA weight {k} has no counterpart in the model state")
+        sd[name] = v
+    return sd
 
 
 # ------------------------------------------------------------------------------------------ the loop
@@ -182,7 +228,10 @@ class Trainer:
                  load_strict_model_weights: bool = True, load_ignore_keys: Sequence[str] = (),
                  log_every: int = 50, log_fn: Callable[[str], None] = print,
                  eval_dataloader: Optional[Iterable[Dict[str, torch.Tensor]]] = None, eval_interval="0ba",
-                 save_num_checkpoints_to_keep: Optional[int] = None):
+                 save_num_checkpoints_to_keep: Optional[int] = None, ema_smoothing: Optional[float] = None,
+                 ema_half_life=None, ema_update_interval="1ba", ema_start="0ba"):
+        """`ema_smoothing` or `ema_half_life` (Composer's EMA arguments, configs/res_512_pretrain.yaml:3-9) keeps an
+        exponential moving average of the weights (ema.FlatEMA) in `self.ema`; without either there is none."""
         import torch.distributed as dist
         self.model = model
         self.loader = train_dataloader
@@ -201,10 +250,13 @@ class Trainer:
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.optimizer = FlatAdamW(model.dit, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, clip_norm=clip_norm)
         self.reducer = GradReducer(model.dit.store, ops=model.dit.engine.ops) if self.world > 1 else None
+        self.ema = (FlatEMA(model.dit, ema_smoothing, ema_half_life, ema_update_interval, ema_start)
+                    if (ema_smoothing is not None or ema_half_life is not None) else None)
         self.batch = 0
         if load_path:
             self.batch = load_checkpoint(load_path, model, self.optimizer, load_weights_only,
-                                         load_strict_model_weights, load_ignore_keys, loader=self.loader, rank=self.rank)
+                                         load_strict_model_weights, load_ignore_keys, loader=self.loader, rank=self.rank,
+                                         ema=self.ema)
 
     def lr_at(self, batch: int) -> float:
         return self.optimizer.lr * lr_multiplier(self.scheduler, batch, self.t_warmup, self.t_max, self.alpha, self.alpha_f)
@@ -213,7 +265,15 @@ class Trainer:
     def evaluate(self) -> float:
         """Composer's eval pass over `eval_dataloader` (trainer.eval_interval, dataset.eval in the configs): mean over
         batches and ranks of `model.eval_forward(batch)`'s loss -- DistLoss (utils.py:598-613: sum of batch losses and a
-        batch count, both sum-reduced across ranks).  The model runs in eval mode (no patch masking, model.py:115-118)."""
+        batch count, both sum-reduced across ranks).  The model runs in eval mode (no patch masking, model.py:115-118).
+        This trainer's rule: once the EMA has started, the pass runs on the EMA weights (`ema.applied()`); the training
+        weights are restored bit for bit afterwards."""
+        if self.ema is not None:
+            with self.ema.applied():
+                return self._evaluate()
+        return self._evaluate()
+
+    def _evaluate(self) -> float:
         import torch.distributed as dist
         dev = self.model.dit.store.device
         was_training = self.model.training
@@ -260,7 +320,7 @@ class Trainer:
                 batch = {k: (v.to(dev, non_blocking=True) if torch.is_tensor(v) else v) for k, v in batch.items()}
                 self.optimizer.lr_now = self.lr_at(self.batch)
                 loss = train_step(self.model, batch, self.optimizer, self.reducer, self.microbatch,
-                                  lr=self.optimizer.lr_now)
+                                  lr=self.optimizer.lr_now, ema=self.ema)
                 self.batch += 1
                 n0 += batch["image_latents"].shape[0] * self.world
                 if self.batch % self.log_every == 0 or self.batch == stop:
@@ -278,7 +338,8 @@ class Trainer:
                 if self.save_folder and self.batch % self.save_interval == 0:
                     self._raise_if_nonfinite()  # never write a checkpoint after a skipped (NaN / Inf) step
                     save_checkpoint(os.path.join(self.save_folder, f"ba{self.batch}.pt"), self.model, self.optimizer,
-                                    self.batch, self.rank, loader=self.loader, world=self.world, keep=self.save_keep)
+                                    self.batch, self.rank, loader=self.loader, world=self.world, keep=self.save_keep,
+                                    ema=self.ema)
                 if self.batch >= stop:
                     break
             if not progressed:
