@@ -145,6 +145,291 @@ __device__ __forceinline__ float2 ld_bf16_pair(const __nv_bfloat16* src, bool tw
   return make_float2(__bfloat162float(src[0]), two ? __bfloat162float(src[1]) : 0.f);
 }
 
+// The tails' arithmetic on one column pair, shared by the guarded and the interior epilogue so that both round the
+// same way.  Bias, gate and residual are separate roundings (__fadd_rn / __fmul_rn): they are never contracted into an
+// FMA with the acc * alpha product, however the code around them is compiled.
+__device__ __forceinline__ void add_pair(float& v0, float& v1, float2 b) {
+  v0 = __fadd_rn(v0, b.x);
+  v1 = __fadd_rn(v1, b.y);
+}
+// C2 = bf16 copy of v (optional, needed by backward for d(gate)); C = v * g (if gated) + r
+__device__ __forceinline__ void resid_tail(float* C, __nv_bfloat16* C2, float v0, float v1, bool gated, float2 g,
+                                           float2 r, bool two, bool vec) {
+  if (C2 != nullptr) st_bf16_pair(C2, v0, v1, two, vec);
+  if (gated) {
+    v0 = __fmul_rn(v0, g.x);
+    v1 = __fmul_rn(v1, g.y);
+  }
+  st_f32_pair(C, __fadd_rn(v0, r.x), __fadd_rn(v1, r.y), two, vec);
+}
+// C = pre-activation (bf16), C2 = act(pre) (bf16); the activation is taken on the bf16-rounded pre-activation so that
+// backward (which re-reads C) differentiates the same function
+template <bool kTanh>
+__device__ __forceinline__ void act_dual_tail(__nv_bfloat16* C, __nv_bfloat16* C2, float v0, float v1, bool two, bool vec) {
+  const float x0 = bf16_round(v0), x1 = bf16_round(v1);
+  st_bf16_pair(C, x0, x1, two, vec);
+  st_bf16_pair(C2, gelu_fast<kTanh>(x0), gelu_fast<kTanh>(x1), two, vec);
+}
+// C = acc * act'(pre): the dgrad GEMM hands the pre-activation gradient on directly
+template <bool kTanh>
+__device__ __forceinline__ void act_grad_tail(__nv_bfloat16* C, float v0, float v1, float2 x, bool two, bool vec) {
+  st_bf16_pair(C, v0 * gelu_grad_fast<kTanh>(x.x), v1 * gelu_grad_fast<kTanh>(x.y), two, vec);
+}
+// u1 = (a0, a1), u2 = (b0, b1) (bias included): du = bf16 u at its interleaved columns (u1 at du, u2 at du + 32),
+// h = silu(u1) * u2 at the natural column
+__device__ __forceinline__ void swiglu_tail(__nv_bfloat16* du, __nv_bfloat16* h, float a0, float a1, float b0, float b1) {
+  a0 = bf16_round(a0); a1 = bf16_round(a1);
+  b0 = bf16_round(b0); b1 = bf16_round(b1);
+  st_bf16_pair(du, a0, a1, true, true);
+  st_bf16_pair(du + 32, b0, b1, true, true);
+  const float h0 = a0 * __fdividef(1.0f, 1.0f + __expf(-a0)) * b0;
+  const float h1 = a1 * __fdividef(1.0f, 1.0f + __expf(-a1)) * b1;
+  st_bf16_pair(h, h0, h1, true, true);
+}
+// d u1 = d h * u2 * silu'(u1) at dst, d u2 = d h * silu(u1) at dst + 32
+__device__ __forceinline__ void swiglu_grad_tail(__nv_bfloat16* dst, float d0, float d1, float2 u1, float2 u2) {
+  const float s0 = __fdividef(1.0f, 1.0f + __expf(-u1.x)), s1 = __fdividef(1.0f, 1.0f + __expf(-u1.y));
+  st_bf16_pair(dst, d0 * u2.x * (s0 * fmaf(u1.x, 1.0f - s0, 1.0f)), d1 * u2.y * (s1 * fmaf(u1.y, 1.0f - s1, 1.0f)),
+               true, true);
+  st_bf16_pair(dst + 32, d0 * u1.x * s0, d1 * u1.y * s1, true, true);
+}
+
+// Epilogue of an interior tile in chunks of CH column groups j (both rows of each).  load(j, side) issues the global
+// loads group j needs into `side`; emit(j, side) does its math and stores.  The loads of the next chunk go out before
+// the math and stores of the current one, so their latencies overlap instead of being waited out one column pair at a
+// time; the first chunk's loads go out before `mma_done` (the wait for the tile's last MMAs: the addresses do not depend
+// on the accumulators).  The batching comes from the source order alone: C may alias a side input (the in-place
+// residual), and every element is still read before it is written.
+template <int NJ, int CH, class Side, class Load, class Emit, class Wait>
+__device__ __forceinline__ void chunked_tail(Load&& load, Emit&& emit, Wait&& mma_done) {
+  static_assert(NJ % CH == 0, "chunks must tile the column groups");
+  Side cur[CH];
+#pragma unroll
+  for (int jj = 0; jj < CH; ++jj) load(jj, cur[jj]);
+  mma_done();
+#pragma unroll
+  for (int j0 = 0; j0 < NJ; j0 += CH) {
+    Side nxt[CH];
+    if (j0 + CH < NJ) {
+#pragma unroll
+      for (int jj = 0; jj < CH; ++jj) load(j0 + CH + jj, nxt[jj]);
+    }
+#pragma unroll
+    for (int jj = 0; jj < CH; ++jj) emit(j0 + jj, cur[jj]);
+    if (j0 + CH < NJ) {
+#pragma unroll
+      for (int jj = 0; jj < CH; ++jj) cur[jj] = nxt[jj];
+    }
+  }
+}
+
+// Side inputs of one column group j (both rows), and how many groups a chunk takes.  Sized so that the 256-wide tile
+// compiles without spills: its 128 accumulators are all live while the first chunk loads, two chunks are live while
+// the next is in flight, and the compiler runs the unrolled math of a chunk side by side (each element's temporaries
+// at once).  Larger chunks for SwiGLU' or GELU' spilled.
+struct BiasSide { float2 b; static constexpr int kChunk = 8; };
+struct ResidSide { float2 b, g[2], r[2]; static constexpr int kChunk = 2; };
+struct SwigluSide { float2 b1, b2; static constexpr int kChunk = 2; };  // groups j % 8 >= 4 load nothing
+template <bool kTanh> struct ActGradSide { __nv_bfloat162 x[2]; static constexpr int kChunk = 4; };
+struct SwigluGradSide { __nv_bfloat162 u1[2], u2[2]; static constexpr int kChunk = 2; };
+
+// Every tail except the atomic one on a tile whose 128 x BLOCK_N elements are all inside the output, with pair accesses
+// allowed everywhere (p.vec2): the same arithmetic as the guarded loops of the kernel, without their per-pair bounds
+// checks and scalar fallbacks.  Thread rows r0, r0 + 8 (i), column pairs cb + 8 j (+0, +1); every access is a per-row
+// base pointer plus a constant offset of j.
+template <int BLOCK_N, class Wait>
+__device__ __forceinline__ void interior_epilogue(const GemmDev& p, float (&acc)[BLOCK_N / 2], int bz, int r0, int cb,
+                                                  Wait&& mma_done) {
+  constexpr int NJ = BLOCK_N / 8;
+  const float alpha = p.alpha;
+  long long crow[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) crow[i] = 1LL * bz * p.strideC + 1LL * (r0 + 8 * i) * p.ldc;
+  auto row_ptr = [&](auto* base, int i) { return base + crow[i] + cb; };
+  const float* bias = p.bias != nullptr ? p.bias + 1LL * bz * p.strideBias + cb : nullptr;
+  auto v = [&](int j, int i, int e) { return acc[4 * j + 2 * i + e] * alpha; };
+  auto ld_bias = [&](int j, BiasSide& s) {
+    if (bias != nullptr) s.b = *reinterpret_cast<const float2*>(bias + 8 * j);
+  };
+  auto with_bias = [&](int j, int i, const BiasSide& s, float& v0, float& v1) {
+    v0 = v(j, i, 0);
+    v1 = v(j, i, 1);
+    if (bias != nullptr) add_pair(v0, v1, s.b);
+  };
+  auto act_kind = [&](auto&& body) {
+    if (p.act) body(std::true_type{});
+    else body(std::false_type{});
+  };
+
+  switch (p.epi) {
+    case EPI_STORE_BF16: {
+      __nv_bfloat16* c[2] = {row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 0), row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 1)};
+      chunked_tail<NJ, BiasSide::kChunk, BiasSide>(ld_bias, [&](int j, const BiasSide& s) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v0, v1;
+          with_bias(j, i, s, v0, v1);
+          st_bf16_pair(c[i] + 8 * j, v0, v1, true, true);
+        }
+      }, mma_done);
+      break;
+    }
+    case EPI_STORE_F32: {
+      float* c[2] = {row_ptr(reinterpret_cast<float*>(p.C), 0), row_ptr(reinterpret_cast<float*>(p.C), 1)};
+      chunked_tail<NJ, BiasSide::kChunk, BiasSide>(ld_bias, [&](int j, const BiasSide& s) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v0, v1;
+          with_bias(j, i, s, v0, v1);
+          st_f32_pair(c[i] + 8 * j, v0, v1, true, true);
+        }
+      }, mma_done);
+      break;
+    }
+    case EPI_RESID_F32: {
+      float* c[2] = {row_ptr(reinterpret_cast<float*>(p.C), 0), row_ptr(reinterpret_cast<float*>(p.C), 1)};
+      __nv_bfloat16* c2[2] = {nullptr, nullptr};
+      const float* res[2];
+      const float* gate[2] = {nullptr, nullptr};
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int row = r0 + 8 * i;
+        if (p.C2 != nullptr) c2[i] = row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C2), i);
+        res[i] = p.res + 1LL * bz * p.strideC + 1LL * (p.res_mod > 0 ? row % p.res_mod : row) * p.ldc + cb;
+        if (p.gate != nullptr) gate[i] = p.gate + 1LL * (row / p.rows_per_gate) * p.ldgate + cb;
+      }
+      // the gate's presence picks the instantiation: a load under a runtime condition would keep a register pair per
+      // group alive on both paths
+      auto gated_kind = [&](auto&& body) {
+        if (p.gate != nullptr) body(std::true_type{});
+        else body(std::false_type{});
+      };
+      gated_kind([&](auto gated_tag) {
+        constexpr bool kGated = decltype(gated_tag)::value;
+        chunked_tail<NJ, ResidSide::kChunk, ResidSide>(
+            [&](int j, ResidSide& s) {
+              if (bias != nullptr) s.b = *reinterpret_cast<const float2*>(bias + 8 * j);
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                if constexpr (kGated) s.g[i] = *reinterpret_cast<const float2*>(gate[i] + 8 * j);
+                s.r[i] = *reinterpret_cast<const float2*>(res[i] + 8 * j);
+              }
+            },
+            [&](int j, const ResidSide& s) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                float v0 = v(j, i, 0), v1 = v(j, i, 1);
+                if (bias != nullptr) add_pair(v0, v1, s.b);
+                resid_tail(c[i] + 8 * j, c2[i] != nullptr ? c2[i] + 8 * j : nullptr, v0, v1, kGated, s.g[i], s.r[i], true,
+                           true);
+              }
+            },
+            mma_done);
+      });
+      break;
+    }
+    case EPI_ACT_DUAL: {
+      __nv_bfloat16* c[2] = {row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 0), row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 1)};
+      __nv_bfloat16* c2[2] = {row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C2), 0), row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C2), 1)};
+      act_kind([&](auto tanh_tag) {
+        constexpr bool kTanh = decltype(tanh_tag)::value;
+        chunked_tail<NJ, BiasSide::kChunk, BiasSide>(ld_bias, [&](int j, const BiasSide& s) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float v0, v1;
+            with_bias(j, i, s, v0, v1);
+            act_dual_tail<kTanh>(c[i] + 8 * j, c2[i] + 8 * j, v0, v1, true, true);
+          }
+        }, mma_done);
+      });
+      break;
+    }
+    case EPI_ACT_GRAD: {
+      __nv_bfloat16* c[2] = {row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 0), row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 1)};
+      const __nv_bfloat16* x[2] = {row_ptr(reinterpret_cast<const __nv_bfloat16*>(p.aux), 0),
+                                   row_ptr(reinterpret_cast<const __nv_bfloat16*>(p.aux), 1)};
+      act_kind([&](auto tanh_tag) {
+        constexpr bool kTanh = decltype(tanh_tag)::value;
+        chunked_tail<NJ, ActGradSide<kTanh>::kChunk, ActGradSide<kTanh>>(
+            [&](int j, ActGradSide<kTanh>& s) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) s.x[i] = *reinterpret_cast<const __nv_bfloat162*>(x[i] + 8 * j);
+            },
+            [&](int j, const ActGradSide<kTanh>& s) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i)
+                act_grad_tail<kTanh>(c[i] + 8 * j, v(j, i, 0), v(j, i, 1), __bfloat1622float2(s.x[i]), true, true);
+            },
+            mma_done);
+      });
+      break;
+    }
+    case EPI_SWIGLU: {
+      // groups j and j + 4 of every 8 hold u1 and u2 of the same columns (see the guarded loop); cb % 64 < 8, so group j
+      // (j % 8 < 4) is column cb + 8 j of u, natural column cb + 8 j - 32 (j / 8) of h and of the bias halves
+      __nv_bfloat16* c[2] = {row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 0), row_ptr(reinterpret_cast<__nv_bfloat16*>(p.C), 1)};
+      __nv_bfloat16* h[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        h[i] = reinterpret_cast<__nv_bfloat16*>(p.C2) + 1LL * bz * p.strideC2 + 1LL * (r0 + 8 * i) * p.ldc2 +
+               (cb >> 6) * 32 + (cb & 63);
+      const float* b1 = p.bias != nullptr ? p.bias + 1LL * bz * p.strideBias + (cb >> 6) * 32 + (cb & 63) : nullptr;
+      chunked_tail<NJ, SwigluSide::kChunk, SwigluSide>(
+          [&](int j, SwigluSide& s) {
+            if ((j & 7) >= 4 || b1 == nullptr) return;
+            s.b1 = *reinterpret_cast<const float2*>(b1 + 8 * j - 32 * (j >> 3));
+            s.b2 = *reinterpret_cast<const float2*>(b1 + 8 * j - 32 * (j >> 3) + (p.N >> 1));
+          },
+          [&](int j, const SwigluSide& s) {
+            if ((j & 7) >= 4) return;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              float a0 = v(j, i, 0), a1 = v(j, i, 1);
+              float bb0 = v(j + 4, i, 0), bb1 = v(j + 4, i, 1);
+              if (b1 != nullptr) {
+                add_pair(a0, a1, s.b1);
+                add_pair(bb0, bb1, s.b2);
+              }
+              swiglu_tail(c[i] + 8 * j, h[i] + 8 * j - 32 * (j >> 3), a0, a1, bb0, bb1);
+            }
+          },
+          mma_done);
+      break;
+    }
+    case EPI_SWIGLU_GRAD: {
+      // dh column n sits at 64 (n / 32) + n % 32 of u and du; cb % 32 < 8, so group j is 64 (j / 4) + 8 (j % 4) further
+      __nv_bfloat16* c[2];
+      const __nv_bfloat16* u[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const long long o = crow[i] + 64 * (cb >> 5) + (cb & 31);
+        c[i] = reinterpret_cast<__nv_bfloat16*>(p.C) + o;
+        u[i] = reinterpret_cast<const __nv_bfloat16*>(p.aux) + o;
+      }
+      auto off = [](int j) { return 64 * (j >> 2) + 8 * (j & 3); };
+      chunked_tail<NJ, SwigluGradSide::kChunk, SwigluGradSide>(
+          [&](int j, SwigluGradSide& s) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              s.u1[i] = *reinterpret_cast<const __nv_bfloat162*>(u[i] + off(j));
+              s.u2[i] = *reinterpret_cast<const __nv_bfloat162*>(u[i] + off(j) + 32);
+            }
+          },
+          [&](int j, const SwigluGradSide& s) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+              swiglu_grad_tail(c[i] + off(j), v(j, i, 0), v(j, i, 1), __bfloat1622float2(s.u1[i]),
+                               __bfloat1622float2(s.u2[i]));
+          },
+          mma_done);
+      break;
+    }
+    default:
+      mma_done();
+      break;
+  }
+}
+
 template <int BLOCK_N, bool kMN>
 __device__ __forceinline__ void wgmma_k16(float (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
   if constexpr (BLOCK_N == 256) wgmma_m64n256k16<kMN ? 1 : 0, kMN ? 1 : 0>(acc, da, db, accumulate);
@@ -267,17 +552,25 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
       }
     }
-    wgmma_wait<0>();
-    wgmma_fence_operands(acc);
-    if (kb1 > kb0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
-    }
+    auto mma_done = [&]() {
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      if (kb1 > kb0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % Cfg::kStages]);
+      }
+    };
 
     // ---------------------------------------------------------------- epilogue, straight from the registers
     // thread owns rows r0, r0 + 8 and column pairs cb + 8 j (+0, +1), j < BLOCK_N / 8
     const int r0 = mb * kBlockM + half * 64 + wq * 16 + (lane >> 2);
     const int cb = nb * BLOCK_N + 2 * (lane & 3);
+    if (vec && p.epi != EPI_ATOMIC_F32 && (mb + 1) * kBlockM <= p.M && (nb + 1) * BLOCK_N <= p.N) {
+      interior_epilogue<BLOCK_N>(p, acc, bz, r0, cb, mma_done);
+      continue;
+    }
+    // edge tiles, unaligned pitches and the atomic tail: every pair checks its bounds and falls back to scalar accesses
+    mma_done();
     // f(row, crow, i, j, col, v0, v1, two) for every in-bounds pair; crow = offset of the output row
     auto for_each_pair = [&](auto&& f) {
 #pragma unroll
@@ -299,11 +592,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     };
     auto add_bias = [&](int col, float& v0, float& v1, bool two) {
-      if (p.bias != nullptr) {
-        const float* b = p.bias + 1LL * bz * p.strideBias + col;
-        v0 += b[0];
-        if (two) v1 += b[1];
-      }
+      if (p.bias != nullptr) add_pair(v0, v1, ld_f32_pair(p.bias + 1LL * bz * p.strideBias + col, two, vec));
     };
 
     switch (p.epi) {
@@ -322,16 +611,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       case EPI_RESID_F32:
         for_each_pair([&](int row, long long crow, int, int, int col, float v0, float v1, bool two) {
           add_bias(col, v0, v1, two);
-          // bf16 copy of the raw GEMM result (needed by backward for d(gate))
-          if (p.C2 != nullptr) st_bf16_pair(reinterpret_cast<__nv_bfloat16*>(p.C2) + crow + col, v0, v1, two, vec);
-          if (p.gate != nullptr) {
-            const float2 g = ld_f32_pair(p.gate + 1LL * (row / p.rows_per_gate) * p.ldgate + col, two, vec);
-            v0 *= g.x;
-            v1 *= g.y;
-          }
+          float2 g = make_float2(0.f, 0.f);
+          if (p.gate != nullptr) g = ld_f32_pair(p.gate + 1LL * (row / p.rows_per_gate) * p.ldgate + col, two, vec);
           const long long rrow = 1LL * bz * p.strideC + 1LL * (p.res_mod > 0 ? row % p.res_mod : row) * p.ldc;
           const float2 r = ld_f32_pair(p.res + rrow + col, two, vec);
-          st_f32_pair(reinterpret_cast<float*>(p.C) + crow + col, v0 + r.x, v1 + r.y, two, vec);
+          resid_tail(reinterpret_cast<float*>(p.C) + crow + col,
+                     p.C2 != nullptr ? reinterpret_cast<__nv_bfloat16*>(p.C2) + crow + col : nullptr, v0, v1,
+                     p.gate != nullptr, g, r, two, vec);
         });
         break;
       case EPI_ATOMIC_F32:
@@ -350,16 +636,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         break;
       case EPI_ACT_DUAL: {
-        // C = pre-activation (bf16), C2 = act(pre) (bf16); the activation is taken on the bf16-rounded pre-activation so
-        // that backward (which re-reads C) differentiates the same function
         auto dual = [&](auto tanh_tag) {
           constexpr bool kTanh = decltype(tanh_tag)::value;
           for_each_pair([&](int, long long crow, int, int, int col, float v0, float v1, bool two) {
             add_bias(col, v0, v1, two);
-            const float x0 = bf16_round(v0), x1 = bf16_round(v1);
-            st_bf16_pair(reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col, x0, x1, two, vec);
-            st_bf16_pair(reinterpret_cast<__nv_bfloat16*>(p.C2) + crow + col, gelu_fast<kTanh>(x0), gelu_fast<kTanh>(x1), two,
-                         vec);
+            act_dual_tail<kTanh>(reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col,
+                                 reinterpret_cast<__nv_bfloat16*>(p.C2) + crow + col, v0, v1, two, vec);
           });
         };
         if (p.act) dual(std::true_type{});
@@ -367,13 +649,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         break;
       }
       case EPI_ACT_GRAD: {
-        // C = acc * act'(pre): the dgrad GEMM hands the pre-activation gradient on directly
         auto grad = [&](auto tanh_tag) {
           constexpr bool kTanh = decltype(tanh_tag)::value;
           for_each_pair([&](int, long long crow, int, int, int col, float v0, float v1, bool two) {
             const float2 x = ld_bf16_pair(reinterpret_cast<const __nv_bfloat16*>(p.aux) + crow + col, two, vec);
-            st_bf16_pair(reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col, v0 * gelu_grad_fast<kTanh>(x.x),
-                         v1 * gelu_grad_fast<kTanh>(x.y), two, vec);
+            act_grad_tail<kTanh>(reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col, v0, v1, x, two, vec);
           });
         };
         if (p.act) grad(std::true_type{});
@@ -393,20 +673,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           float b0 = acc[4 * (j + 4) + 2 * i] * alpha, b1 = acc[4 * (j + 4) + 2 * i + 1] * alpha;
           if (p.bias != nullptr) {
             const float* bb = p.bias + 1LL * bz * p.strideBias + 32 * (col >> 6) + (col & 63);
-            const float2 x1 = ld_f32_pair(bb, true, vec), x2 = ld_f32_pair(bb + (p.N >> 1), true, vec);
-            a0 += x1.x; a1 += x1.y;
-            b0 += x2.x; b1 += x2.y;
+            add_pair(a0, a1, ld_f32_pair(bb, true, vec));
+            add_pair(b0, b1, ld_f32_pair(bb + (p.N >> 1), true, vec));
           }
-          a0 = bf16_round(a0); a1 = bf16_round(a1);
-          b0 = bf16_round(b0); b1 = bf16_round(b1);
-          __nv_bfloat16* du = reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col;
-          st_bf16_pair(du, a0, a1, true, true);
-          st_bf16_pair(du + 32, b0, b1, true, true);
-          const float h0 = a0 * __fdividef(1.0f, 1.0f + __expf(-a0)) * b0;
-          const float h1 = a1 * __fdividef(1.0f, 1.0f + __expf(-a1)) * b1;
-          st_bf16_pair(reinterpret_cast<__nv_bfloat16*>(p.C2) + 1LL * bz * p.strideC2 + 1LL * row * p.ldc2 +
-                           (col >> 6) * 32 + (col & 63),
-                       h0, h1, true, true);
+          swiglu_tail(reinterpret_cast<__nv_bfloat16*>(p.C) + crow + col,
+                      reinterpret_cast<__nv_bfloat16*>(p.C2) + 1LL * bz * p.strideC2 + 1LL * row * p.ldc2 +
+                          (col >> 6) * 32 + (col & 63),
+                      a0, a1, b0, b1);
         });
         break;
       case EPI_SWIGLU_GRAD:
@@ -417,11 +690,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const long long off = crow + 64 * (col >> 5) + (col & 31);
           const float2 u1 = ld_bf16_pair(reinterpret_cast<const __nv_bfloat16*>(p.aux) + off, true, true);
           const float2 u2 = ld_bf16_pair(reinterpret_cast<const __nv_bfloat16*>(p.aux) + off + 32, true, true);
-          const float s0 = __fdividef(1.0f, 1.0f + __expf(-u1.x)), s1 = __fdividef(1.0f, 1.0f + __expf(-u1.y));
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + off;
-          st_bf16_pair(dst, d0 * u2.x * (s0 * fmaf(u1.x, 1.0f - s0, 1.0f)), d1 * u2.y * (s1 * fmaf(u1.y, 1.0f - s1, 1.0f)),
-                       true, true);
-          st_bf16_pair(dst + 32, d0 * u1.x * s0, d1 * u1.y * s1, true, true);
+          swiglu_grad_tail(reinterpret_cast<__nv_bfloat16*>(p.C) + off, d0, d1, u1, u2);
         });
         break;
       default:
