@@ -1,11 +1,12 @@
 // Non-causal multi-head attention forward / backward for short sequences (T in {64, 77, 256, 1024}),
-// head_dim 32 or 64: F.scaled_dot_product_attention at utils.py:188-193 (self) and utils.py:127-132
+// head_dim 32, 64 or 128: F.scaled_dot_product_attention at utils.py:188-193 (self) and utils.py:127-132
 // (cross, 77 caption tokens) and its autograd backward.
 //
 // This file: the mma.sync kernels -- flash-style tiles of 64 queries x 64 keys per CTA (4 warps x 16 rows), bf16
 // mma.sync m16n8k16 with fp32 accumulation and online softmax in the log2 domain; backward is the deterministic
-// two-kernel split (dK/dV per key tile, dQ per query tile; no atomics) plus fused few-key variants.  md_attn_fwd runs
-// them for head_dim 32 and more than 256 keys, md_attn_bwd for head_dim 32 and up to 128 keys (the rest: attn_wgmma.cu).
+// two-kernel split (dK/dV per key tile, dQ per query tile; no atomics) plus fused few-key variants (head_dim 32 / 64;
+// head_dim 128 always takes the split).  md_attn_fwd runs them for head_dim 32, head_dim 64 beyond 256 keys and
+// unaligned operands; md_attn_bwd for head_dim 32 / 128 and head_dim 64 up to 128 keys (the rest: attn_wgmma.cu).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -119,6 +120,27 @@ __device__ __forceinline__ void mma_p_m(float (&out)[HD / 8][4], const uint32_t 
       ldsm_x4_t(b, m + (kt * 16 + (lane & 7) + (mi & 1) * 8) * Smem<HD>::kPitch + dp * 16 + (mi >> 1) * 8);
       mma16816(out[2 * dp], pa[kt], b[0], b[1]);
       mma16816(out[2 * dp + 1], pa[kt], b[2], b[3]);
+    }
+  }
+}
+
+// mma_a_bt with the A operand (16 x HD, smem rows r0..r0+15) read from shared memory one k-step at a time instead of
+// held in registers: what the dK / dV kernel needs at head_dim 128, where K / V fragments next to the dK / dV
+// accumulators would not fit in the register file.
+template <int HD, int KT = kTile>
+__device__ __forceinline__ void mma_sa_bt(float (&acc)[KT / 8][4], const __nv_bfloat16* sa, int r0, const __nv_bfloat16* m,
+                                          int lane) {
+#pragma unroll
+  for (int ks = 0; ks < HD / 16; ++ks) {
+    uint32_t a[4];
+    ldsm_x4(a, sa + (r0 + (lane & 15)) * Smem<HD>::kPitch + ks * 16 + (lane >> 4) * 8);
+#pragma unroll
+    for (int np = 0; np < KT / 16; ++np) {
+      uint32_t b[4];
+      const int mi = lane >> 3;
+      ldsm_x4(b, m + (np * 16 + (lane & 7) + (mi >> 1) * 8) * Smem<HD>::kPitch + ks * 16 + (mi & 1) * 8);
+      mma16816(acc[2 * np], a, b[0], b[1]);
+      mma16816(acc[2 * np + 1], a, b[2], b[3]);
     }
   }
 }
@@ -251,7 +273,7 @@ template <int HD>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, long long lddo, const __nv_bfloat16* __restrict__ o,
                   long long ldo, float* __restrict__ delta, long long rows, int H, int Tq) {
-  constexpr int kLanesPerHead = HD / 8;  // 8 (HD=64) or 4 (HD=32)
+  constexpr int kLanesPerHead = HD / 8;  // 16 (HD=128), 8 (HD=64) or 4 (HD=32)
   constexpr int kMaxChunks = 8;          // uint4 chunks per lane: H*HD <= 2048
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunks = H * kLanesPerHead;
@@ -322,9 +344,14 @@ attn_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ dout, long long lddo, con
   load_tile<HD>(sk, k + b * Tk * ldk, ldk, k0, Tk, h * HD);
   load_tile<HD>(sv, v + b * Tk * ldv, ldv, k0, Tk, h * HD);
   __syncthreads();
+  // head_dim 128: the K / V A fragments stay in shared memory (read per k-step), so that the 2 x 64 dK / dV accumulators
+  // and the S^T / dP^T tiles fit in registers without spilling
+  constexpr bool kFragsInSmem = HD == 128;
   uint32_t ka[HD / 16][4], va[HD / 16][4];
-  load_a_frags<HD>(ka, sk, warp * 16, lane);
-  load_a_frags<HD>(va, sv, warp * 16, lane);
+  if constexpr (!kFragsInSmem) {
+    load_a_frags<HD>(ka, sk, warp * 16, lane);
+    load_a_frags<HD>(va, sv, warp * 16, lane);
+  }
 
   float dkacc[HD / 8][4], dvacc[HD / 8][4];
 #pragma unroll
@@ -349,8 +376,13 @@ attn_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ dout, long long lddo, con
     for (int i = 0; i < 8; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) st[i][j] = dpt[i][j] = 0.f;
-    mma_a_bt<HD>(st, ka, sq, lane);    // S^T  = K . Q^T     (16 keys x 64 queries)
-    mma_a_bt<HD>(dpt, va, sdo, lane);  // dP^T = V . dO^T
+    if constexpr (kFragsInSmem) {
+      mma_sa_bt<HD>(st, sk, warp * 16, sq, lane);
+      mma_sa_bt<HD>(dpt, sv, warp * 16, sdo, lane);
+    } else {
+      mma_a_bt<HD>(st, ka, sq, lane);    // S^T  = K . Q^T     (16 keys x 64 queries)
+      mma_a_bt<HD>(dpt, va, sdo, lane);  // dP^T = V . dO^T
+    }
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -818,7 +850,8 @@ static size_t small_bwd_smem() {
 }
 
 static int check_attn(const char* what, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd, int64_t ld_min) {
-  if (hd != 32 && hd != 64) return md_set_error(MD_ERR_UNSUPPORTED, "attention: head_dim must be 32 or 64");
+  if (hd != 32 && hd != 64 && hd != 128)
+    return md_set_error(MD_ERR_UNSUPPORTED, "attention: head_dim must be 32, 64 or 128");
   if (B < 0 || H <= 0 || Tq <= 0 || Tk <= 0 || H > 65535 || B > 65535)
     return md_set_error(MD_ERR_INVALID, what);
   if (ld_min % 8 != 0) return md_set_error(MD_ERR_INVALID, "attention: row pitches must be multiples of 8 elements");
@@ -844,10 +877,13 @@ extern "C" int md_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ld
   if (B == 0) return 0;
   if (!q || !k || !v || !o || !lse) return md_set_error(MD_ERR_INVALID, "md_attn_fwd: null pointer");
   // head_dim 64 with all keys in one S tile: the wgmma kernel (attn_wgmma.cu), 1.3-1.5x faster than mma.sync on every
-  // forward shape of the res-256 configs on an H100 (B = 256, H = 12 / 16, Tq x Tk = 256 x 256 / 64 x 64 / 64 x 77 / 256 x 77)
+  // forward shape of the res-256 configs on an H100 (B = 256, H = 12 / 16, Tq x Tk = 256 x 256 / 64 x 64 / 64 x 77 / 256 x 77).
+  // head_dim 128, any Tk: the chunked wgmma kernel, 1.5-2.5x faster than attn_fwd_kernel<128, .> on every measured shape
+  // (res-256 and res-512 MicroDiT_XL_2 widths, 64-1024 queries, 64-1024 keys; DESIGN.md 5.2), so it always takes it.
   const uintptr_t align = reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
                           reinterpret_cast<uintptr_t>(o);
-  if (hd == 64 && Tk <= 256 && (align & 15) == 0 && ((ldq | ldk | ldv | ldo) % 8) == 0)
+  const bool tc_ok = (align & 15) == 0 && ((ldq | ldk | ldv | ldo) % 8) == 0;
+  if (tc_ok && ((hd == 64 && Tk <= 256) || hd == 128))
     return md_attn_fwd_tc(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tk, hd, stream);
   return md_attn_fwd_mma(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tk, hd, stream);
 }
@@ -872,7 +908,8 @@ extern "C" int md_attn_fwd_mma(const void* q, int64_t ldq, const void* k, int64_
     attn_fwd_kernel<HD_, KT_><<<grid, 128, sm, ST(stream)>>>(CBF(q), ldq, CBF(k), ldk, CBF(v), ldv, BF(o), ldo, lse, \
                                                              (int)H, (int)Tq, (int)Tk, sl2);                         \
   } while (0)
-  if (hd == 64) { if (kt80) FWD(64, 80); else FWD(64, 64); }
+  if (hd == 128) { if (kt80) FWD(128, 80); else FWD(128, 64); }
+  else if (hd == 64) { if (kt80) FWD(64, 80); else FWD(64, 64); }
   else { if (kt80) FWD(32, 80); else FWD(32, 64); }
 #undef FWD
   return check_launch("md_attn_fwd");
@@ -909,7 +946,8 @@ extern "C" int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, in
     return md_set_error(MD_ERR_INVALID, "md_attn_bwd: null pointer");
   const float scale = 1.f / sqrtf((float)hd);
   const float sl2 = 1.4426950408889634f * scale;
-  if (Tq <= kTile && Tk <= 80) {  // single-pass fused backward
+  // head_dim 128 always takes the generic split below: the fused few-key kernels are laid out for <= 64 columns
+  if (hd != 128 && Tq <= kTile && Tk <= 80) {  // single-pass fused backward
     dim3 gs((unsigned)H, (unsigned)B);
 #define BWD_SMALL(HD_, KT_)                                                                                          \
   do {                                                                                                               \
@@ -928,7 +966,7 @@ extern "C" int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, in
 #undef BWD_SMALL
     return check_launch("md_attn_bwd");
   }
-  if (Tk <= 80) {  // few keys, many queries (cross-attention at T = 256 / 1024): K / V resident, dK / dV in registers
+  if (hd != 128 && Tk <= 80) {  // few keys, many queries (cross-attention at T = 256 / 1024): K / V resident, dK / dV in registers
     dim3 gs((unsigned)H, (unsigned)B);
 #define BWD_CROSS(HD_, KT_)                                                                                          \
   do {                                                                                                               \
@@ -947,10 +985,14 @@ extern "C" int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, in
 #undef BWD_CROSS
     return check_launch("md_attn_bwd");
   }
+  // the delta kernel holds a whole token row (all heads) in one warp: H*hd <= 2048, i.e. at most 16 heads at head_dim 128
   if (H * hd > 2048) return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_bwd: H*hd must be <= 2048");
   long long blocks = (B * Tq + 7) / 8;
   if (blocks > 132 * 8) blocks = 132 * 8;
-  if (hd == 64)
+  if (hd == 128)
+    attn_delta_kernel<128><<<(unsigned)blocks, 256, 0, ST(stream)>>>(CBF(dout), lddo, CBF(o), ldo, delta, B * Tq, (int)H,
+                                                                     (int)Tq);
+  else if (hd == 64)
     attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, ST(stream)>>>(CBF(dout), lddo, CBF(o), ldo, delta, B * Tq, (int)H,
                                                                     (int)Tq);
   else
@@ -975,7 +1017,7 @@ extern "C" int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, in
                                                             lse, delta, BF(dq), lddq, (int)H, (int)Tq, (int)Tk,      \
                                                             scale, sl2);                                             \
   } while (0)
-  if (hd == 64) BWD_GENERIC(64); else BWD_GENERIC(32);
+  if (hd == 128) BWD_GENERIC(128); else if (hd == 64) BWD_GENERIC(64); else BWD_GENERIC(32);
 #undef BWD_GENERIC
   return check_launch("md_attn_bwd");
 }

@@ -5,7 +5,9 @@
 // column-slice operands with row pitches, lse in the log2 domain, delta = rowsum(dO * O) written to the scratch.
 //
 // One warp per query row (forward, dQ) or per key row (dK / dV): lanes take one key (query) each for the score, then
-// the weighted sum over the 32 scores is accumulated with each lane owning head_dim / 32 output columns.
+// the weighted sum over the 32 scores is accumulated with each lane owning head_dim / 32 output columns.  The backward
+// kernels read two whole rows in every lane (q and dO, or k and v); up to head_dim 64 they sit in registers, at 128 they
+// would spill, so there they live in a per-warp shared-memory copy that the lanes read by broadcast.
 #include "common.cuh"
 
 namespace md {
@@ -80,13 +82,28 @@ dq_kernel(const float* __restrict__ dout, long long lddo, const float* __restric
   const float* qr = q + (b * Tq + qi) * ldq + h * HD;
   const float* dor = dout + (b * Tq + qi) * lddo + h * HD;
   const float* orow = o + (b * Tq + qi) * ldo + h * HD;
-  float qv[HD], dov[HD];
+  constexpr bool kSmemRows = HD == 128;
+  __shared__ float srows[kSmemRows ? 4 * 2 * HD : 1];
+  float qreg[kSmemRows ? 1 : HD], doreg[kSmemRows ? 1 : HD];
+  float* qv = kSmemRows ? srows + (threadIdx.x >> 5) * 2 * HD : qreg;
+  float* dov = kSmemRows ? qv + HD : doreg;
   float dl = 0.f;
+  if constexpr (kSmemRows) {
 #pragma unroll
-  for (int d = 0; d < HD; ++d) {
-    qv[d] = qr[d] * scale;
-    dov[d] = dor[d];
-    dl = fmaf(dov[d], orow[d], dl);
+    for (int e = 0; e < DPL; ++e) {
+      qv[lane + 32 * e] = qr[lane + 32 * e] * scale;
+      dov[lane + 32 * e] = dor[lane + 32 * e];
+    }
+    __syncwarp();
+#pragma unroll
+    for (int d = 0; d < HD; ++d) dl = fmaf(dov[d], orow[d], dl);
+  } else {
+#pragma unroll
+    for (int d = 0; d < HD; ++d) {
+      qv[d] = qr[d] * scale;
+      dov[d] = dor[d];
+      dl = fmaf(dov[d], orow[d], dl);
+    }
   }
   const float lrow = lse[(b * H + h) * Tq + qi];
   if (lane == 0) delta[(b * H + h) * Tq + qi] = dl;
@@ -137,11 +154,24 @@ dkdv_kernel(const float* __restrict__ dout, long long lddo, const float* __restr
   const long long b = w / (1LL * Tk * H);
   const float* kr = k + (b * Tk + kj) * ldk + h * HD;
   const float* vr = v + (b * Tk + kj) * ldv + h * HD;
-  float kv[HD], vv[HD];
+  constexpr bool kSmemRows = HD == 128;
+  __shared__ float srows[kSmemRows ? 4 * 2 * HD : 1];
+  float kreg[kSmemRows ? 1 : HD], vreg[kSmemRows ? 1 : HD];
+  float* kv = kSmemRows ? srows + (threadIdx.x >> 5) * 2 * HD : kreg;
+  float* vv = kSmemRows ? kv + HD : vreg;
+  if constexpr (kSmemRows) {
 #pragma unroll
-  for (int d = 0; d < HD; ++d) {
-    kv[d] = kr[d] * scale;
-    vv[d] = vr[d];
+    for (int e = 0; e < DPL; ++e) {
+      kv[lane + 32 * e] = kr[lane + 32 * e] * scale;
+      vv[lane + 32 * e] = vr[lane + 32 * e];
+    }
+    __syncwarp();
+  } else {
+#pragma unroll
+    for (int d = 0; d < HD; ++d) {
+      kv[d] = kr[d] * scale;
+      vv[d] = vr[d];
+    }
   }
   float ak[DPL], av[DPL];
 #pragma unroll
@@ -195,12 +225,16 @@ extern "C" int md_attn_fwd_f32(const void* q, int64_t ldq, const void* k, int64_
                                int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd,
                                void* stream) {
   if (B <= 0 || H <= 0 || Tq <= 0 || Tk <= 0) return B == 0 ? 0 : md_set_error(MD_ERR_INVALID, "md_attn_fwd_f32: bad sizes");
-  if (hd != 32 && hd != 64) return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_fwd_f32: head_dim must be 32 or 64");
+  if (hd != 32 && hd != 64 && hd != 128)
+    return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_fwd_f32: head_dim must be 32, 64 or 128");
   if (!q || !k || !v || !o || !lse) return md_set_error(MD_ERR_INVALID, "md_attn_fwd_f32: null pointer");
   const long long rows = B * H * Tq;
   const unsigned grid = static_cast<unsigned>((rows + 3) / 4);
   const float scale = 1.f / sqrtf(static_cast<float>(hd));
-  if (hd == 64)
+  if (hd == 128)
+    attn_f32::fwd_kernel<128><<<grid, 128, 0, ST(stream)>>>(CF(q), ldq, CF(k), ldk, CF(v), ldv, F(o), ldo, lse, (int)H, (int)Tq,
+                                                            (int)Tk, rows, scale);
+  else if (hd == 64)
     attn_f32::fwd_kernel<64><<<grid, 128, 0, ST(stream)>>>(CF(q), ldq, CF(k), ldk, CF(v), ldv, F(o), ldo, lse, (int)H, (int)Tq,
                                                            (int)Tk, rows, scale);
   else
@@ -214,7 +248,8 @@ extern "C" int md_attn_bwd_f32(const void* dout, int64_t lddo, const void* q, in
                                void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
                                int64_t Tq, int64_t Tk, int64_t hd, void* stream) {
   if (B <= 0 || H <= 0 || Tq <= 0 || Tk <= 0) return B == 0 ? 0 : md_set_error(MD_ERR_INVALID, "md_attn_bwd_f32: bad sizes");
-  if (hd != 32 && hd != 64) return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_bwd_f32: head_dim must be 32 or 64");
+  if (hd != 32 && hd != 64 && hd != 128)
+    return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_bwd_f32: head_dim must be 32, 64 or 128");
   if (!dout || !q || !k || !v || !o || !lse || !delta || !dq || !dk || !dv)
     return md_set_error(MD_ERR_INVALID, "md_attn_bwd_f32: null pointer");
   const long long qrows = B * H * Tq, krows = B * H * Tk;
@@ -228,7 +263,8 @@ extern "C" int md_attn_bwd_f32(const void* dout, int64_t lddo, const void* q, in
         CF(dout), lddo, CF(q), ldq, CF(k), ldk, CF(v), ldv, lse, delta, F(dk), lddk, F(dv), lddv, (int)H, (int)Tq,     \
         (int)Tk, krows, scale);                                                                                        \
   } while (0)
-  if (hd == 64) BWD(64);
+  if (hd == 128) BWD(128);
+  else if (hd == 64) BWD(64);
   else BWD(32);
 #undef BWD
   return check_launch("md_attn_bwd_f32");

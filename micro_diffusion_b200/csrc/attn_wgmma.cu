@@ -1,5 +1,5 @@
-// Attention on the Hopper warpgroup tensor cores (TMA + wgmma) for head_dim 64: forward for Tk <= 256 (below), backward
-// for any Tk (further down).
+// Attention on the Hopper warpgroup tensor cores (TMA + wgmma): forward for head_dim 64 and Tk <= 256 (below), forward
+// for head_dim 128 and any Tk (after it), backward for head_dim 64 and any Tk (further down).
 //
 // Contract = md_attn_fwd: softmax(Q K^T / sqrt(hd)) V, non-causal (F.scaled_dot_product_attention at reference
 // utils.py:188-193 self, 127-132 cross); q / k / v are column slices of the packed projection buffers; lse in the
@@ -169,6 +169,178 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   }
 }
 
+// ------------------------------------------------------------------------------------------ head_dim 128 forward
+// Same contract for head_dim 128 and any Tk.  All keys of a head in one S tile no longer fit next to a 64 x 128 O
+// accumulator (a 64 x 256 S tile alone is 128 fp32 registers per thread), so this kernel runs an online softmax over
+// 64-key chunks (log2 domain, the running max rescales l and O per chunk, as in the mma.sync kernels).
+//
+// One CTA = one warpgroup = 64 query rows of one (sample, head).  Every 64-column half of a 128-column row is its own
+// 128B-swizzled TMA box (64 rows x 128 B), so Q is two boxes and each key chunk is two K boxes and two V boxes.  K / V
+// chunks stream through a two-stage ring: chunk c + 2 is loaded into the stage of chunk c once every warp is done with
+// it, so the load of chunk c + 1 overlaps the math of chunk c.  S = Q K^T of a chunk is 8 k16 steps of m64n64k16 (the
+// first four in the first column box); O += P V is two m64n64k16 chains (one per 64-column half of O) with P as the
+// register A operand, V read MN-major.  126 registers, no spills, 81 KB of shared memory: two CTAs per SM.
+constexpr int kHd128 = 128;
+constexpr int kBox = 64 * 64 * 2;                       // one 64-row x 64-column bf16 box: 8 KB
+constexpr int k128OffKV = 2 * kBox;                     // Q: two boxes
+constexpr int k128Stage = 4 * kBox;                     // K (two boxes) | V (two boxes)
+constexpr int k128OffBar = k128OffKV + 2 * k128Stage;   // two stages
+constexpr int k128SmemBytes = k128OffBar + 64 + 1024;
+
+__global__ void __launch_bounds__(128)
+attn_fwd_wgmma128_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                         const __grid_constant__ CUtensorMap tmV, __nv_bfloat16* __restrict__ o, long long ldo,
+                         float* __restrict__ lse, int H, int Tq, int Tk, float sl2) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + k128OffBar);  // one barrier per stage
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int nc = (Tk + 63) >> 6;  // 64-key chunks
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int col0 = h * kHd128;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    mbar_init(&full[0], 1);
+    mbar_init(&full[1], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  // issued by thread 0: key chunk c (and Q with the first) into stage c & 1, zero-filled past Tq / Tk
+  auto load_chunk = [&](int c) {
+    uint8_t* st = smem + k128OffKV + (c & 1) * k128Stage;
+    uint64_t* bar = &full[c & 1];
+    mbar_expect_tx(bar, k128Stage + (c == 0 ? 2 * kBox : 0));
+    if (c == 0) {
+      tma_load_3d(&tmQ, bar, smem, col0, qb * kQ, b);
+      tma_load_3d(&tmQ, bar, smem + kBox, col0 + 64, qb * kQ, b);
+    }
+    tma_load_3d(&tmK, bar, st, col0, c * 64, b);
+    tma_load_3d(&tmK, bar, st + kBox, col0 + 64, c * 64, b);
+    tma_load_3d(&tmV, bar, st + 2 * kBox, col0, c * 64, b);
+    tma_load_3d(&tmV, bar, st + 3 * kBox, col0 + 64, c * 64, b);
+  };
+  if (threadIdx.x == 0) {
+    load_chunk(0);
+    if (nc > 1) load_chunk(1);
+  }
+
+  // fragment of thread t: rows r0 = 16 warp + lane / 4 and r0 + 8 (i = 0, 1), columns 8 j + 2 (lane % 4) + e of
+  // s[4 j + 2 i + e] (keys of the chunk) and of o[half][4 j + 2 i + e] (head columns 64 half + ...)
+  const int cq = 2 * (lane & 3);
+  float oacc[2][32];
+#pragma unroll
+  for (int x = 0; x < 2; ++x)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) oacc[x][i] = 0.f;
+  float m2[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // running max (log2 domain) and per-thread partial sum
+  const uint32_t sq = smem_u32(smem);
+
+  for (int c = 0; c < nc; ++c) {
+    const uint8_t* st = smem + k128OffKV + (c & 1) * k128Stage;
+    mbar_wait(&full[c & 1], (c >> 1) & 1);
+
+    // ---- S = Q K^T over the 128 head columns: k16 steps 0..3 in the first column box, 4..7 in the second
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kHd128 / 16; ++k) {
+      const uint64_t dq = wgmma_smem_desc(sq + (k >> 2) * kBox, 16, 1024) + 2 * (k & 3);
+      const uint64_t dk = wgmma_smem_desc(smem_u32(st) + (k >> 2) * kBox, 16, 1024) + 2 * (k & 3);
+      wgmma_m64n64k16<0, 0>(s, dq, dk, k > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
+
+    // ---- online softmax: mask keys past Tk, new running max, rescale of l and O
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * j + 2 * i + e];
+          if (c * 64 + 8 * j + cq + e >= Tk) v = -INFINITY;
+          mx[i] = fmaxf(mx[i], v);
+        }
+    float corr[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      const float mn = fmaxf(m2[i], mx[i] * sl2);  // every chunk has a valid key: finite
+      corr[i] = ex2_approx(m2[i] - mn);             // first chunk: exp2(-inf) = 0
+      m2[i] = mn;
+      l[i] *= corr[i];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * j + 2 * i + e];
+          v = ex2_approx(fmaf(v, sl2, -m2[i]));
+          l[i] += v;
+        }
+#pragma unroll
+    for (int x = 0; x < 2; ++x)
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          oacc[x][4 * j + 2 * i] *= corr[i];
+          oacc[x][4 * j + 2 * i + 1] *= corr[i];
+        }
+
+    // ---- O += P V: P (bf16) from registers, V MN-major (head columns contiguous), 16-key steps 2048 B apart
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) pa[t][r] = pack2(s[8 * t + 2 * r], s[8 * t + 2 * r + 1]);
+    const uint64_t dv0 = wgmma_smem_desc(smem_u32(st + 2 * kBox), 64 * 128, 1024);
+    const uint64_t dv1 = wgmma_smem_desc(smem_u32(st + 3 * kBox), 64 * 128, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      wgmma_m64n64k16_rs<1>(oacc[0], pa[t], dv0 + static_cast<uint64_t>(t * 128), 1u);
+      wgmma_m64n64k16_rs<1>(oacc[1], pa[t], dv1 + static_cast<uint64_t>(t * 128), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(oacc[0]);
+    wgmma_fence_operands(oacc[1]);
+    __syncthreads();  // every warp is done with this stage before chunk c + 2 lands in it
+    if (threadIdx.x == 0 && c + 2 < nc) load_chunk(c + 2);
+  }
+
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = qb * kQ + warp * 16 + (lane >> 2) + 8 * i;
+    if (row < Tq) {
+      const float inv = __fdividef(1.f, l[i]);
+      __nv_bfloat16* dst = o + (static_cast<long long>(b) * Tq + row) * ldo + col0 + cq;
+#pragma unroll
+      for (int x = 0; x < 2; ++x)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint32_t*>(dst + 64 * x + 8 * j) =
+              pack2(oacc[x][4 * j + 2 * i] * inv, oacc[x][4 * j + 2 * i + 1] * inv);
+      if ((lane & 3) == 0) lse[(static_cast<long long>(b) * H + h) * Tq + row] = m2[i] + __log2f(l[i]);
+    }
+  }
+}
+
 // bf16 [batch][rows][cols] view, box = [1][box_rows][64 columns], 128B swizzle.
 int make_map(CUtensorMap* map, const void* ptr, long long cols, long long rows, long long batch, long long ld,
              int box_rows) {
@@ -188,15 +360,33 @@ extern "C" int md_attn_fwd_tc(const void* q, int64_t ldq, const void* k, int64_t
   using namespace md;
   using namespace md::attn_wg;
   if (B <= 0 || H <= 0 || Tq <= 0 || Tk <= 0) return B == 0 ? 0 : md_set_error(MD_ERR_INVALID, "md_attn_fwd_tc: bad sizes");
-  if (hd != kHd || Tk > kMaxKeys)
-    return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_fwd_tc: needs head_dim 64 and Tk <= 256");
+  if (!(hd == kHd && Tk <= kMaxKeys) && hd != kHd128)
+    return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_fwd_tc: needs head_dim 64 with Tk <= 256, or head_dim 128");
   if (!q || !k || !v || !o || !lse) return md_set_error(MD_ERR_INVALID, "md_attn_fwd_tc: null pointer");
   const uintptr_t align = reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
                           reinterpret_cast<uintptr_t>(o);
   if ((align & 15) != 0 || ((ldq | ldk | ldv | ldo) % 8) != 0)
     return md_set_error(MD_ERR_INVALID, "md_attn_fwd_tc: operands must be 16-byte aligned with pitches % 8 == 0");
-  const int kbox = static_cast<int>((Tk + 63) / 64 * 64);
   CUtensorMap tmQ, tmK, tmV;
+  const dim3 grid(static_cast<unsigned>((Tq + kQ - 1) / kQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
+  const float sl2 = 1.4426950408889634f / sqrtf(static_cast<float>(hd));
+  if (hd == kHd128) {
+    if (int rc = make_map(&tmQ, q, H * hd, Tq, B, ldq, kQ)) return rc;
+    if (int rc = make_map(&tmK, k, H * hd, Tk, B, ldk, 64)) return rc;
+    if (int rc = make_map(&tmV, v, H * hd, Tk, B, ldv, 64)) return rc;
+    static bool attr128 = false;
+    if (!attr128) {
+      cudaError_t e =
+          cudaFuncSetAttribute(attn_fwd_wgmma128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, k128SmemBytes);
+      if (e != cudaSuccess) return md_set_error(MD_ERR_CUDA, cudaGetErrorString(e));
+      attr128 = true;
+    }
+    attn_fwd_wgmma128_kernel<<<grid, 128, k128SmemBytes, reinterpret_cast<cudaStream_t>(stream)>>>(
+        tmQ, tmK, tmV, reinterpret_cast<__nv_bfloat16*>(o), ldo, lse, static_cast<int>(H), static_cast<int>(Tq),
+        static_cast<int>(Tk), sl2);
+    return check_launch("md_attn_fwd_tc");
+  }
+  const int kbox = static_cast<int>((Tk + 63) / 64 * 64);
   if (int rc = make_map(&tmQ, q, H * hd, Tq, B, ldq, kQ)) return rc;
   if (int rc = make_map(&tmK, k, H * hd, Tk, B, ldk, kbox)) return rc;
   if (int rc = make_map(&tmV, v, H * hd, Tk, B, ldv, kbox)) return rc;
@@ -206,8 +396,6 @@ extern "C" int md_attn_fwd_tc(const void* q, int64_t ldq, const void* k, int64_t
     if (e != cudaSuccess) return md_set_error(MD_ERR_CUDA, cudaGetErrorString(e));
     attr = true;
   }
-  const dim3 grid(static_cast<unsigned>((Tq + kQ - 1) / kQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  const float sl2 = 1.4426950408889634f / sqrtf(static_cast<float>(hd));
   attn_fwd_wgmma_kernel<<<grid, 128, kSmemBytes, reinterpret_cast<cudaStream_t>(stream)>>>(
       tmQ, tmK, tmV, reinterpret_cast<__nv_bfloat16*>(o), ldo, lse, static_cast<int>(H), static_cast<int>(Tq),
       static_cast<int>(Tk), sl2);

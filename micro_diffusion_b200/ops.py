@@ -135,8 +135,9 @@ class CudaOps:
             self.set_deterministic(True)
         self.gemm_flops = 0      # algorithmic FLOPs of every md_gemm_bf16 launched (2*M*N*K*batch)
         # None: md_attn_fwd chooses the forward kernel per shape; True: the wgmma kernel (md_attn_fwd_tc) wherever its
-        # envelope allows (head_dim 64, Tk <= 256) and the wgmma backward (md_attn_bwd_tc, head_dim 64); False: the
-        # mma.sync kernels (md_attn_fwd_mma / md_attn_bwd_mma), for A/B runs.
+        # envelope allows (head_dim 64 with Tk <= 256, or head_dim 128) and the wgmma backward (md_attn_bwd_tc, head_dim
+        # 64; head_dim 128 has none and takes md_attn_bwd); False: the mma.sync kernels (md_attn_fwd_mma /
+        # md_attn_bwd_mma), for A/B runs.
         self.attn_tc = None
         self.sm_limit = 0        # > 0: persistent GEMM grids use at most this many SMs (set while a collective overlaps)
         self.profile = None      # set to a list to record (name, start_event, end_event, flops) per launch
@@ -349,7 +350,8 @@ class CudaOps:
         if self.prec:
             name = "md_attn_fwd_f32"
         else:
-            name = "md_attn_fwd_tc" if (self.attn_tc and hd == 64 and Tk <= 256) else "md_attn_fwd"
+            tc_ok = (hd == 64 and Tk <= 256) or hd == 128
+            name = "md_attn_fwd_tc" if (self.attn_tc and tc_ok) else "md_attn_fwd"
             if self.attn_tc is False:
                 name = "md_attn_fwd_mma"
         self._call(name, q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
