@@ -307,7 +307,11 @@ extern "C" int md_edm_loss_fwd(const float* ftok, const int32_t* keep_tok, const
   if (B == 0) return 0;
   if (!ftok || !lat || !xn || !coef || !per_sample || !loss)
     return md_set_error(MD_ERR_INVALID, "md_edm_loss_fwd: null pointer");
-  float* ws = det_enabled() ? det_workspace(static_cast<size_t>(B) * sizeof(float)) : nullptr;
+  float* ws = nullptr;
+  if (det_enabled()) {  // B > 262144 samples overflow the 1 MiB minimum workspace: refuse rather than take the atomics
+    ws = det_workspace(static_cast<size_t>(B) * sizeof(float));
+    if (ws == nullptr) return md_set_error(MD_ERR_INVALID, "md_edm_loss_fwd: deterministic workspace too small");
+  }
   edm_loss_kernel<false, float><<<(unsigned)B, 256, 0, ST(stream)>>>(ftok, keep_tok, lat, lat_f16, xn, coef, per_sample,
                                                                      loss, nullptr, nullptr, (int)B, (int)C, (int)H,
                                                                      (int)W, (int)p, (int)Tk, ws);

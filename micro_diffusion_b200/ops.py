@@ -263,7 +263,8 @@ class CudaOps:
         a.lda, a.ldb, a.ldc = A3.stride(1), B3.stride(1), C3.stride(1)
         a.batch = A3.shape[0]
         a.strideA, a.strideB, a.strideC = A3.stride(0), B3.stride(0), C3.stride(0)
-        a.strideBias = bias.stride(0) if (bias is not None and bias.dim() == 2) else N
+        # [batch, N]: one bias per batch entry; [N]: one bias shared by every batch entry (stride 0)
+        a.strideBias = bias.stride(0) if (bias is not None and bias.dim() == 2) else 0
         a.gate, a.ldgate = _mod(gate)
         a.rows_per_gate = rows_per_gate
         a.res_mod = res_mod
