@@ -147,19 +147,22 @@ MD_API int md_gate_bwd(const float* dres, const void* y, const float* gate, int6
 /* ------------------------------------------------------------------------------------- attention */
 /* softmax(Q K^T / sqrt(hd)) V, non-causal (F.scaled_dot_product_attention at utils.py:188-193 self,
  * 127-132 cross).  q [B*Tq, *] pitch ldq, k / v [B*Tk, *] pitch ldk / ldv, head h at column h*hd;
- * o bf16 [B*Tq, H*hd] pitch ldo; lse f32 [B,H,Tq] (log2 domain).  hd 32, 64 or 128 (any other: MD_ERR_UNSUPPORTED). */
+ * o bf16 [B*Tq, H*hd] pitch ldo; lse f32 [B,H,Tq] (log2 domain).  hd 32, 64 or 128 (any other: MD_ERR_UNSUPPORTED).
+ * Every bf16 attention entry point needs q / k / v / o (and dout / dq / dk / dv) 16-byte aligned and every row pitch a
+ * multiple of 8 elements; anything else is MD_ERR_INVALID. */
 MD_API int md_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                        int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd,
                        void* stream);
-/* delta scratch f32 [B,H,Tq]; dq/dk/dv bf16 with the pitches of q/k/v.  hd 32, 64 or 128; where the generic
- * dK / dV + dQ split runs (every hd-128 shape, and more than 80 keys at hd 32 / 64) H*hd must be <= 2048: at most 16 heads
- * at hd 128. */
+/* delta scratch f32 [B,H,Tq]; dq/dk/dv bf16 with the pitches of q/k/v.  hd 32, 64 or 128; where the backward runs a
+ * delta pass (every hd-128 shape, and more than 80 keys at hd 32 / 64) H*hd must be <= 2048: at most 16 heads at hd 128,
+ * 32 at hd 64. */
 MD_API int md_attn_bwd(const void* dout, int64_t lddo, const void* q, int64_t ldq, const void* k, int64_t ldk,
                        const void* v, int64_t ldv, const void* o, int64_t ldo, const float* lse, float* delta,
                        void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
                        int64_t Tq, int64_t Tk, int64_t hd, void* stream);
 /* The same backward on wgmma (csrc/attn_wgmma.cu) for head_dim 64, any Tk: a dK / dV kernel role per 64-key block and a
- * dQ role per 64-query block (no atomics); delta is scratch.  md_attn_bwd dispatches here above 128 keys. */
+ * dQ role per 64-query block (no atomics); delta is scratch.  md_attn_bwd dispatches here above 128 keys.  H*hd must be
+ * <= 2048 (at most 32 heads), as for the generic split; more is MD_ERR_UNSUPPORTED. */
 MD_API int md_attn_bwd_tc(const void* dout, int64_t lddo, const void* q, int64_t ldq, const void* k, int64_t ldk,
                           const void* v, int64_t ldv, const void* o, int64_t ldo, const float* lse, float* delta,
                           void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
@@ -176,7 +179,7 @@ MD_API int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, int64_
 /* The same forward on the warpgroup tensor cores (TMA + wgmma, csrc/attn_wgmma.cu) for head_dim 64 with Tk <= 256 (one
  * 64-query tile per CTA, whole-row softmax in registers, P fed back to the tensor core from registers) and for head_dim
  * 128 with any Tk (online softmax over 64-key chunks streamed through a two-stage TMA ring).  md_attn_fwd dispatches here
- * whenever the shape is inside this envelope and the operands are 16-byte aligned. */
+ * whenever the shape is inside this envelope. */
 MD_API int md_attn_fwd_tc(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                           int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd,
                           void* stream);

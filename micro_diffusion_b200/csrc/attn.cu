@@ -5,9 +5,12 @@
 // This file: the mma.sync kernels -- flash-style tiles of 64 queries x 64 keys per CTA (4 warps x 16 rows), bf16
 // mma.sync m16n8k16 with fp32 accumulation and online softmax in the log2 domain; backward is the deterministic
 // two-kernel split (dK/dV per key tile, dQ per query tile; no atomics) plus fused few-key variants (head_dim 32 / 64;
-// head_dim 128 always takes the split).  md_attn_fwd runs them for head_dim 32, head_dim 64 beyond 256 keys and
-// unaligned operands; md_attn_bwd for head_dim 32 / 128 and head_dim 64 up to 128 keys (the rest: attn_wgmma.cu).
+// head_dim 128 always takes the split).  md_attn_fwd runs them for head_dim 32 and head_dim 64 beyond 256 keys;
+// md_attn_bwd for head_dim 32 / 128 and head_dim 64 up to 128 keys (the rest: attn_wgmma.cu).  Every entry point
+// requires 16-byte aligned operands: the tiles move in 16-byte loads (uint4, cp.async 16).
 #include <stdlib.h>
+
+#include <initializer_list>
 
 #include "common.cuh"
 
@@ -849,13 +852,23 @@ static size_t small_bwd_smem() {
   return sizeof(__nv_bfloat16) * (HD == 64 ? base : base + 2 * kTile * (KT + 8));
 }
 
-static int check_attn(const char* what, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd, int64_t ld_min) {
+// lds: every row pitch or'ed together; ptrs: every operand address or'ed together.  Each row of a head is read and
+// written in 16-byte pieces, so both must keep 16-byte alignment.
+static int check_attn(const char* what, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd, int64_t lds,
+                      uintptr_t ptrs) {
   if (hd != 32 && hd != 64 && hd != 128)
     return md_set_error(MD_ERR_UNSUPPORTED, "attention: head_dim must be 32, 64 or 128");
   if (B < 0 || H <= 0 || Tq <= 0 || Tk <= 0 || H > 65535 || B > 65535)
     return md_set_error(MD_ERR_INVALID, what);
-  if (ld_min % 8 != 0) return md_set_error(MD_ERR_INVALID, "attention: row pitches must be multiples of 8 elements");
+  if (lds % 8 != 0) return md_set_error(MD_ERR_INVALID, "attention: row pitches must be multiples of 8 elements");
+  if ((ptrs & 15) != 0) return md_set_error(MD_ERR_INVALID, "attention: operands must be 16-byte aligned");
   return 0;
+}
+
+static uintptr_t addr_or(std::initializer_list<const void*> ps) {
+  uintptr_t a = 0;
+  for (const void* p : ps) a |= reinterpret_cast<uintptr_t>(p);
+  return a;
 }
 
 }  // namespace md
@@ -873,17 +886,15 @@ using namespace md;
 extern "C" int md_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                            int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd,
                            void* stream) {
-  if (int rc = check_attn("md_attn_fwd: bad sizes", B, H, Tq, Tk, hd, (ldq | ldk | ldv | ldo))) return rc;
+  if (int rc = check_attn("md_attn_fwd: bad sizes", B, H, Tq, Tk, hd, (ldq | ldk | ldv | ldo), addr_or({q, k, v, o})))
+    return rc;
   if (B == 0) return 0;
   if (!q || !k || !v || !o || !lse) return md_set_error(MD_ERR_INVALID, "md_attn_fwd: null pointer");
   // head_dim 64 with all keys in one S tile: the wgmma kernel (attn_wgmma.cu), 1.3-1.5x faster than mma.sync on every
   // forward shape of the res-256 configs on an H100 (B = 256, H = 12 / 16, Tq x Tk = 256 x 256 / 64 x 64 / 64 x 77 / 256 x 77).
   // head_dim 128, any Tk: the chunked wgmma kernel, 1.5-2.5x faster than attn_fwd_kernel<128, .> on every measured shape
   // (res-256 and res-512 MicroDiT_XL_2 widths, 64-1024 queries, 64-1024 keys; DESIGN.md 5.2), so it always takes it.
-  const uintptr_t align = reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
-                          reinterpret_cast<uintptr_t>(o);
-  const bool tc_ok = (align & 15) == 0 && ((ldq | ldk | ldv | ldo) % 8) == 0;
-  if (tc_ok && ((hd == 64 && Tk <= 256) || hd == 128))
+  if ((hd == 64 && Tk <= 256) || hd == 128)
     return md_attn_fwd_tc(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tk, hd, stream);
   return md_attn_fwd_mma(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tk, hd, stream);
 }
@@ -891,7 +902,8 @@ extern "C" int md_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ld
 extern "C" int md_attn_fwd_mma(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                                int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tk, int64_t hd,
                                void* stream) {
-  if (int rc = check_attn("md_attn_fwd: bad sizes", B, H, Tq, Tk, hd, (ldq | ldk | ldv | ldo))) return rc;
+  if (int rc = check_attn("md_attn_fwd: bad sizes", B, H, Tq, Tk, hd, (ldq | ldk | ldv | ldo), addr_or({q, k, v, o})))
+    return rc;
   if (B == 0) return 0;
   if (!q || !k || !v || !o || !lse) return md_set_error(MD_ERR_INVALID, "md_attn_fwd: null pointer");
   const float sl2 = 1.4426950408889634f / sqrtf((float)hd);
@@ -919,16 +931,14 @@ extern "C" int md_attn_bwd(const void* dout, int64_t lddo, const void* q, int64_
                            const void* v, int64_t ldv, const void* o, int64_t ldo, const float* lse, float* delta,
                            void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
                            int64_t Tq, int64_t Tk, int64_t hd, void* stream) {
-  if (int rc = check_attn("md_attn_bwd: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv)))
+  if (int rc = check_attn("md_attn_bwd: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv),
+                          addr_or({dout, q, k, v, o, dq, dk, dv})))
     return rc;
   if (B == 0) return 0;
   if (!dout || !q || !k || !v || !o || !lse || !delta || !dq || !dk || !dv)
     return md_set_error(MD_ERR_INVALID, "md_attn_bwd: null pointer");
   // head_dim 64 beyond 128 keys: the wgmma backward (attn_wgmma.cu); up to 128 keys the fused few-key mma.sync kernels
-  const uintptr_t align = reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
-                          reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) |
-                          reinterpret_cast<uintptr_t>(dv);
-  if (hd == 64 && Tk > 128 && (align & 15) == 0)
+  if (hd == 64 && Tk > 128)
     return md_attn_bwd_tc(dout, lddo, q, ldq, k, ldk, v, ldv, o, ldo, lse, delta, dq, lddq, dk, lddk, dv, lddv, B, H, Tq, Tk,
                           hd, stream);
   return md_attn_bwd_mma(dout, lddo, q, ldq, k, ldk, v, ldv, o, ldo, lse, delta, dq, lddq, dk, lddk, dv, lddv, B, H, Tq, Tk, hd,
@@ -939,7 +949,8 @@ extern "C" int md_attn_bwd_mma(const void* dout, int64_t lddo, const void* q, in
                                const void* v, int64_t ldv, const void* o, int64_t ldo, const float* lse, float* delta,
                                void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
                                int64_t Tq, int64_t Tk, int64_t hd, void* stream) {
-  if (int rc = check_attn("md_attn_bwd: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv)))
+  if (int rc = check_attn("md_attn_bwd: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv),
+                          addr_or({dout, q, k, v, o, dq, dk, dv})))
     return rc;
   if (B == 0) return 0;
   if (!dout || !q || !k || !v || !o || !lse || !delta || !dq || !dk || !dv)
@@ -1026,16 +1037,15 @@ extern "C" int md_attn_bwd_tc(const void* dout, int64_t lddo, const void* q, int
                               const void* v, int64_t ldv, const void* o, int64_t ldo, const float* lse, float* delta,
                               void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H,
                               int64_t Tq, int64_t Tk, int64_t hd, void* stream) {
-  if (int rc = check_attn("md_attn_bwd_tc: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv)))
+  if (int rc = check_attn("md_attn_bwd_tc: bad sizes", B, H, Tq, Tk, hd, (lddo | ldq | ldk | ldv | ldo | lddq | lddk | lddv),
+                          addr_or({dout, q, k, v, o, dq, dk, dv})))
     return rc;
   if (B == 0) return 0;
   if (hd != 64) return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_bwd_tc: needs head_dim 64");
   if (!dout || !q || !k || !v || !o || !lse || !delta || !dq || !dk || !dv)
     return md_set_error(MD_ERR_INVALID, "md_attn_bwd_tc: null pointer");
-  const uintptr_t align = reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
-                          reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) |
-                          reinterpret_cast<uintptr_t>(dv);
-  if ((align & 15) != 0) return md_set_error(MD_ERR_INVALID, "md_attn_bwd_tc: operands must be 16-byte aligned");
+  // the delta kernel holds a whole token row (all heads) in one warp: H*hd <= 2048, i.e. at most 32 heads of 64
+  if (H * hd > 2048) return md_set_error(MD_ERR_UNSUPPORTED, "md_attn_bwd_tc: H*hd must be <= 2048");
   long long blocks = (B * Tq + 7) / 8;
   if (blocks > 132 * 8) blocks = 132 * 8;
   attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, ST(stream)>>>(CBF(dout), lddo, CBF(o), ldo, delta, B * Tq, (int)H, (int)Tq);
