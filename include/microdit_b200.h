@@ -59,7 +59,8 @@ MD_API int md_set_deterministic(void* workspace, int64_t bytes);
 #define MD_EPI_STORE_F32 1  /* C(f32)  = alpha*acc (+bias)                                           */
 #define MD_EPI_RESID_F32 2  /* C(f32)  = res[row % res_mod] + gate[row/rows_per_gate]*(alpha*acc+bias) */
                             /*           C2(bf16, optional) = alpha*acc+bias                         */
-#define MD_EPI_ATOMIC_F32 3 /* C(f32) += alpha*acc   (red.global.add; the only mode allowing splits) */
+#define MD_EPI_ATOMIC_F32 3 /* C(f32) += alpha*acc   (red.global.add; the only mode allowing splits; no bias:
+                             * a bias is MD_ERR_INVALID) */
 #define MD_EPI_ACT_DUAL 4   /* C(bf16) = pre = alpha*acc+bias ; C2(bf16) = act(pre); act: 0 gelu-erf, 1 gelu-tanh */
 #define MD_EPI_ACT_GRAD 5   /* C(bf16) = alpha*acc * act'(aux) (no bias): the dgrad GEMM of an activation's output applies the
                              * activation's derivative at the saved pre-activation aux (bf16, indexed like C) */

@@ -787,6 +787,9 @@ extern "C" int md_gemm_bf16(const md_gemm_args* a, void* stream_) {
     return md_set_error(MD_ERR_INVALID, "md_gemm_bf16: activation-gradient epilogue needs aux (the saved pre-activation)");
   if (a->epilogue == EPI_ACT_GRAD && a->bias != nullptr)
     return md_set_error(MD_ERR_INVALID, "md_gemm_bf16: the activation-gradient epilogue takes no bias");
+  // every split would add it once (and the deterministic partials not at all): C += alpha*acc has no bias term
+  if (a->epilogue == EPI_ATOMIC_F32 && a->bias != nullptr)
+    return md_set_error(MD_ERR_INVALID, "md_gemm_bf16: the accumulate epilogue takes no bias");
   if (a->epilogue == EPI_SWIGLU || a->epilogue == EPI_SWIGLU_GRAD) {
     const bool fwd = a->epilogue == EPI_SWIGLU;
     const void* second = fwd ? a->C2 : a->aux;

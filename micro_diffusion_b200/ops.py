@@ -279,7 +279,8 @@ class CudaOps:
             a.ldc2 = C2.stride(-2)
             a.strideC2 = C2.stride(0) if C2.dim() == 3 else 0
         elif C2 is not None:
-            assert C2.is_contiguous() or C2.stride(-2) == C3.stride(1)
+            # the kernel writes C2 at C's offsets (batch stride, row pitch): any other layout lands in the wrong place
+            assert C2.shape == Cm.shape and C2.stride() == Cm.stride(), (C2.shape, C2.stride(), Cm.shape, Cm.stride())
         if aux is not None:
             assert aux.dtype == torch.bfloat16 and aux.shape == Cm.shape and aux.stride() == Cm.stride()
         if res is not None:

@@ -87,7 +87,7 @@ class EmuOps:
             assert Cm.dtype == torch.float32
             C3.copy_(acc)
         elif epi == EPI_ATOMIC:
-            assert Cm.dtype == torch.float32
+            assert Cm.dtype == torch.float32 and bias is None, "the accumulate epilogue takes no bias"
             if row_interleave:  # rows arrive in the 32-interleaved order of a w1 | w2 stack, the gradient is in parameter order
                 C3.index_add_(1, interleave_perm(row_interleave), acc)
             else:

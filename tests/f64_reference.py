@@ -72,7 +72,9 @@ def gemm(A, B, layout=0, *, alpha=1.0, bias=None, res=None, res_mod=0, gate=None
       * accumulate (EPI_ATOMIC): accumulate + acc;
       * res (EPI_RESID): res[m % res_mod] + gate[m // rows_per_gate] * acc;
       * act with aux (EPI_ACT_GRAD): acc * gelu'(aux);  act alone (EPI_ACT_DUAL): (acc, gelu(acc)).
-    bias is [N] or [batch, N]."""
+    bias is [N] or [batch, N]; the accumulate epilogue takes none."""
+    if accumulate is not None and bias is not None:
+        raise ValueError("the accumulate epilogue (EPI_ATOMIC) takes no bias")
     acc = matmul(A, B, layout) * (alpha if alpha != 0 else 1.0)
     if bias is not None:
         b = f64(bias)

@@ -254,11 +254,12 @@ def _ops(mode):
     return ops
 
 
-def _traced(ops, fn, want, attempts=4):
-    """fn()'s result, the C entry points it called and the attention kernels it launched.  A short profiler session
-    now and then loses kernel records of a call that did run (a few of ~500 sessions per run, sometimes two in a row).
-    fn has no effect beyond its fresh outputs, so a session whose kernels are not `want` is traced again, up to
-    `attempts` times, and printed with what it did record; a dispatch that really differs fails every attempt."""
+def _traced(ops, fn, want, attempts=4, keep="attn", ids=_kernel_ids):
+    """fn()'s result, the C entry points it called and the kernels it launched whose names contain one of `keep`
+    (a string or a tuple of strings); ids(names) maps them to (kernel ids, unrecognised names).  A short profiler
+    session now and then loses kernel records of a call that did run (a few of ~500 sessions per run, sometimes two in
+    a row).  fn has no effect beyond its fresh outputs, so a session whose kernels are not `want` is traced again, up
+    to `attempts` times, and printed with what it did record; a dispatch that really differs fails every attempt."""
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
     orig = ops._call
@@ -277,8 +278,8 @@ def _traced(ops, fn, want, attempts=4):
             ops._call = orig
         # the raw kernel records, not prof.events(): nothing here needs them matched to the CPU ops that launched them
         device = [e.name() for e in prof.profiler.kineto_results.events() if e.device_type() == DeviceType.CUDA]
-        names = {n for n in device if "attn" in n}
-        if _kernel_ids(names) == (want, []) or attempt == attempts - 1:
+        names = {n for n in device if any(k in n for k in ((keep,) if isinstance(keep, str) else keep))}
+        if ids(names) == (want, []) or attempt == attempts - 1:
             return out, calls, names
         print(f"\n[trace {attempt}: {calls}, {sorted(names)} among {len(device)} device records]", end="")
         time.sleep(0.2)
