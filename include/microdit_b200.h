@@ -290,6 +290,28 @@ MD_API int md_edm_loss_bwd(const float* ftok, const int32_t* keep_tok, const voi
 MD_API int md_edm_output(const float* ftok, const int32_t* ids_restore, const float* mask_token, const float* xn,
                          const float* coef, float* fx, float* dx, int64_t B, int64_t C, int64_t H, int64_t W,
                          int64_t p, int64_t Tk, void* stream);
+/* One stage of the fp64 Heun sampler (LatentDiffusion._heun, model.py:260-276) on the state x, x_hat, d_cur (f64
+ * [B * sample_numel] each).  The step k is read from *step (device int32) and t_cur = table[k], t_next = table[k+1],
+ * t_hat = table[max_steps+1+k] from table (device f64 [2*max_steps+1]), so one captured graph serves every step.
+ *   stage 0 (in):      x_hat = x + sqrt(t_hat^2 - t_cur^2) * s_noise * noise[k]   (noise f64 [max_steps, B*sample_numel])
+ *   stage 1 (euler):   d_cur = (x_hat - den) / t_hat; x = x_hat + (t_next - t_hat) * d_cur
+ *   stage 2 (correct): x = x_hat + (t_next - t_hat) * (0.5 * d_cur + 0.5 * (x - den) / t_next)
+ *   stage 3 (next):    *step += 1 (one thread; only `step` is read)
+ * Stages 0 and 1 also write the next denoiser input: xin f32 = the new x_hat / x, `copies` (1, or 2 for a CFG batch) times
+ * back to back, and sigma f32 [copies*B] = t_hat / t_next.  den: f32 [B * sample_numel] denoiser output.  Every operation
+ * is rounded on its own in the association order of the torch expressions (no FMA contraction), so the result is bit-for-bit
+ * the eager loop's.  A step index outside [0, max_steps) writes NaN instead of reading outside the table. */
+MD_API int md_edm_heun(int stage, double* x, double* x_hat, double* d_cur, const float* den, const double* noise,
+                       float* xin, float* sigma, const double* table, int32_t* step, int64_t max_steps, int64_t B,
+                       int64_t sample_numel, int64_t copies, double s_noise, void* stream);
+/* Classifier-free guidance + EDM preconditioning of a doubled batch (model.py:197-201): ftok f32 [2B*T, p*p*C] holds the
+ * cond samples [0, B) then the uncond samples [B, 2B) (no masking), x f32 [B,C,H,W] the denoiser input, sigma f32 [B],
+ * cfg f32 [1] (device) the guidance scale.  dx = c_skip*x + c_out*(unc + cfg*(cond - unc)) with c_skip =
+ * (1 / (sigma^2 + sigma_data_sq)) * sigma_data_sq and c_out = sigma*sigma_data / sqrt(sigma^2 + sigma_data_sq), each
+ * operation rounded on its own like the torch expression it replaces. */
+MD_API int md_edm_output_cfg(const float* ftok, const float* x, const float* sigma, const float* cfg, float* dx,
+                             float sigma_data, float sigma_data_sq, int64_t B, int64_t C, int64_t H, int64_t W, int64_t p,
+                             void* stream);
 
 /* ----------------------------------------------- adjoints for the differentiable DiT.forward (VJP) */
 /* adjoint of the unmask_tokens + unpatchify of md_edm_output for the raw output F (utils.py:417-426,

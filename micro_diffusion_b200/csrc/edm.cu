@@ -265,6 +265,80 @@ __global__ void gather_rows_kernel(const float* __restrict__ x, const int32_t* _
   }
 }
 
+// ------------------------------------------------------------------------------------- EDM Heun sampler
+// The fp64 state update of LatentDiffusion._heun (model.py:260-276), one launch per stage, so that one captured CUDA graph
+// serves every step: the per-step times come from a device table and a device step index that the graph advances itself.
+// table f64 [2*max_steps + 1] = [t_steps[0..max_steps] | t_hat[0..max_steps)].  Every operation is an explicitly rounded
+// intrinsic in the association order of the torch expressions, so nothing is contracted into an FMA and the state is
+// bit-identical to the eager loop's.
+enum { HEUN_IN = 0, HEUN_EULER = 1, HEUN_CORRECT = 2, HEUN_NEXT = 3 };
+
+__global__ void edm_heun_kernel(int stage, double* __restrict__ x, double* __restrict__ x_hat, double* __restrict__ d_cur,
+                                const float* __restrict__ den, const double* __restrict__ noise, float* __restrict__ xin,
+                                float* __restrict__ sigma, const double* __restrict__ table,
+                                const int32_t* __restrict__ step, int max_steps, long long n, int B, int copies,
+                                double s_noise) {
+  const int k = *step;
+  const bool ok = k >= 0 && k < max_steps;  // an index outside the table poisons the outputs instead of reading past it
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  const double t_cur = ok ? table[k] : nan, t_next = ok ? table[k + 1] : nan, t_hat = ok ? table[max_steps + 1 + k] : nan;
+  const long long tid = 1LL * blockIdx.x * blockDim.x + threadIdx.x;
+  if (stage != HEUN_CORRECT && tid < 1LL * copies * B)
+    sigma[tid] = __double2float_rn(stage == HEUN_IN ? t_hat : t_next);  // t_hat / t_next .to(float32), per sample
+  // (t_hat ** 2 - t_cur ** 2).sqrt() * S_noise and t_next - t_hat: 0-dim tensors in the eager loop
+  const double c_noise = __dmul_rn(__dsqrt_rn(__dsub_rn(__dmul_rn(t_hat, t_hat), __dmul_rn(t_cur, t_cur))), s_noise);
+  const double dt = __dsub_rn(t_next, t_hat);
+  for (long long i = tid; i < n; i += 1LL * gridDim.x * blockDim.x) {
+    double out;
+    if (stage == HEUN_IN) {  // x_hat = x_cur + c * n_k
+      out = __dadd_rn(x[i], __dmul_rn(c_noise, ok ? noise[1LL * k * n + i] : nan));
+      x_hat[i] = out;
+    } else if (stage == HEUN_EULER) {  // d_cur = (x_hat - D) / t_hat; x_next = x_hat + (t_next - t_hat) * d_cur
+      const double xh = x_hat[i];
+      const double d = __ddiv_rn(__dsub_rn(xh, static_cast<double>(den[i])), t_hat);
+      d_cur[i] = d;
+      out = __dadd_rn(xh, __dmul_rn(dt, d));
+      x[i] = out;
+    } else {  // d' = (x_next - D) / t_next; x_next = x_hat + (t_next - t_hat) * (0.5 * d_cur + 0.5 * d')
+      const double dp = __ddiv_rn(__dsub_rn(x[i], static_cast<double>(den[i])), t_next);
+      x[i] = __dadd_rn(x_hat[i], __dmul_rn(dt, __dadd_rn(__dmul_rn(0.5, d_cur[i]), __dmul_rn(0.5, dp))));
+      continue;
+    }
+    const float f = __double2float_rn(out);  // the next denoiser input, in both halves of a CFG batch
+    xin[i] = f;
+    if (copies == 2) xin[n + i] = f;
+  }
+}
+
+__global__ void edm_heun_next_kernel(int32_t* step) { *step += 1; }
+
+// Classifier-free guidance + preconditioning for the doubled batch (model.py:197-201): ftok holds the cond samples
+// [0, B) then the uncond samples [B, 2B).  D = c_skip * x + c_out * (unc + cfg * (cond - unc)) with the rounding of the
+// torch expression: c_skip = reciprocal(sg*sg + sd2) * sd2 (a Python float over a tensor is a reciprocal and a product),
+// c_out = (sg * sd) / sqrt(sg*sg + sd2), every product and sum rounded on its own.
+__global__ void edm_output_cfg_kernel(const float* __restrict__ ftok, const float* __restrict__ x,
+                                      const float* __restrict__ sigma, const float* __restrict__ cfg,
+                                      float* __restrict__ dx, float sd, float sd2, int B, int C, int H, int W, int p) {
+  const int gw = W / p, T = gw * (H / p), Nf = p * p * C;
+  const long long total = 1LL * B * C * H * W;
+  const float g = *cfg;
+  for (long long i = 1LL * blockIdx.x * blockDim.x + threadIdx.x; i < total; i += 1LL * gridDim.x * blockDim.x) {
+    const int xx = static_cast<int>(i % W);
+    long long r = i / W;
+    const int y = static_cast<int>(r % H); r /= H;
+    const int c = static_cast<int>(r % C);
+    const int b = static_cast<int>(r / C);
+    const long long col = ((y % p) * p + (xx % p)) * C + c, tok = (y / p) * gw + xx / p;
+    const float cond = ftok[(1LL * b * T + tok) * Nf + col], unc = ftok[(1LL * (B + b) * T + tok) * Nf + col];
+    const float f = __fadd_rn(unc, __fmul_rn(g, __fsub_rn(cond, unc)));
+    const float sg = sigma[b];
+    const float den = __fadd_rn(__fmul_rn(sg, sg), sd2);
+    const float c_skip = __fmul_rn(__frcp_rn(den), sd2);
+    const float c_out = __fdiv_rn(__fmul_rn(sg, sd), __fsqrt_rn(den));
+    dx[i] = __fadd_rn(__fmul_rn(c_skip, x[i]), __fmul_rn(c_out, f));
+  }
+}
+
 static int grid_for(long long items, int threads) {
   long long blocks = (items + threads - 1) / threads;
   if (blocks > 132LL * 16) blocks = 132LL * 16;
@@ -405,4 +479,40 @@ extern "C" int md_scatter_rows_f32(const float* dy, const int32_t* src_rows, flo
   if (!dy || !src_rows || !dx || D % 4 != 0) return md_set_error(MD_ERR_INVALID, "md_scatter_rows_f32: bad argument");
   gather_rows_kernel<<<grid_for(rows * (D / 4), 256), 256, 0, ST(stream)>>>(dy, src_rows, dx, rows, (int)D, 1);
   return check_launch("md_scatter_rows_f32");
+}
+
+extern "C" int md_edm_heun(int stage, double* x, double* x_hat, double* d_cur, const float* den, const double* noise,
+                           float* xin, float* sigma, const double* table, int32_t* step, int64_t max_steps, int64_t B,
+                           int64_t sample_numel, int64_t copies, double s_noise, void* stream) {
+  if (stage < HEUN_IN || stage > HEUN_NEXT) return md_set_error(MD_ERR_INVALID, "md_edm_heun: stage must be 0..3");
+  if (!step) return md_set_error(MD_ERR_INVALID, "md_edm_heun: null pointer");
+  if (stage == HEUN_NEXT) {
+    edm_heun_next_kernel<<<1, 1, 0, ST(stream)>>>(step);
+    return check_launch("md_edm_heun");
+  }
+  if (max_steps < 1 || max_steps > (1 << 20)) return md_set_error(MD_ERR_INVALID, "md_edm_heun: max_steps out of range");
+  if (B < 1 || sample_numel < 1 || (copies != 1 && copies != 2))
+    return md_set_error(MD_ERR_INVALID, "md_edm_heun: B and sample_numel must be >= 1, copies 1 or 2");
+  if (!table || !x || !x_hat) return md_set_error(MD_ERR_INVALID, "md_edm_heun: null pointer");
+  if (stage == HEUN_IN && (!noise || !xin || !sigma)) return md_set_error(MD_ERR_INVALID, "md_edm_heun: null pointer");
+  if (stage == HEUN_EULER && (!d_cur || !den || !xin || !sigma))
+    return md_set_error(MD_ERR_INVALID, "md_edm_heun: null pointer");
+  if (stage == HEUN_CORRECT && (!d_cur || !den)) return md_set_error(MD_ERR_INVALID, "md_edm_heun: null pointer");
+  const long long n = B * sample_numel;
+  edm_heun_kernel<<<grid_for(n, 256), 256, 0, ST(stream)>>>(stage, x, x_hat, d_cur, den, noise, xin, sigma, table, step,
+                                                            (int)max_steps, n, (int)B, (int)copies, s_noise);
+  return check_launch("md_edm_heun");
+}
+
+extern "C" int md_edm_output_cfg(const float* ftok, const float* x, const float* sigma, const float* cfg, float* dx,
+                                 float sigma_data, float sigma_data_sq, int64_t B, int64_t C, int64_t H, int64_t W,
+                                 int64_t p, void* stream) {
+  if (B == 0) return 0;
+  if (!ftok || !x || !sigma || !cfg || !dx) return md_set_error(MD_ERR_INVALID, "md_edm_output_cfg: null pointer");
+  if (B < 0 || C < 1 || p <= 0 || H % p != 0 || W % p != 0)
+    return md_set_error(MD_ERR_INVALID, "md_edm_output_cfg: bad shape (H, W must be multiples of p)");
+  edm_output_cfg_kernel<<<grid_for(B * C * H * W, 256), 256, 0, ST(stream)>>>(ftok, x, sigma, cfg, dx, sigma_data,
+                                                                             sigma_data_sq, (int)B, (int)C, (int)H,
+                                                                             (int)W, (int)p);
+  return check_launch("md_edm_output_cfg");
 }

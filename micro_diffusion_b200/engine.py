@@ -35,6 +35,7 @@ class Engine:
         # gated-residual backward of the next branch emitted by the preceding LayerNorm backward (A/B knob)
         self.fuse_ln = os.environ.get("MD_FUSE_LN", "1") != "0"
         self.L = None  # caption length, set per call
+        self._sampler_graphs = {}
 
     # ================================================================== helpers
     # True while backward_output(param_grads=False) runs: every weight-gradient GEMM, bias column sum and LayerNorm
@@ -659,6 +660,31 @@ class Engine:
         o.edm_output(c.ftok, c.ids_restore, self.mask_token.reshape(-1), c.xn, c.coef, fx, dx, self.cfg.patch_size, c.Tk)
         return dx, fx, c.mask
 
+    def denoise_cfg(self, x2, sigma2, cfg, edm, prompt):
+        """model_forward_wrapper's guided branch (model.py:188-202) without gradients: the denoiser on the doubled batch
+        x2 = [x; x] with the prompt cache of [caption; zeros], then guidance and preconditioning in one kernel.  cfg: f32 [1]
+        on the device.  Returns D f32 [B,C,H,W]."""
+        o = self.ops
+        c = self._denoiser_fwd(x2, o.zeros(tuple(x2.shape), F32), None, sigma2, None, None, 0.0, None, edm, keep=False,
+                               prompt=prompt)
+        B = x2.shape[0] // 2
+        dx = o.empty((B, *x2.shape[1:]), F32)
+        o.edm_output_cfg(c.ftok, x2[:B], sigma2, cfg, dx, edm["sigma_data"], self.cfg.patch_size)
+        return dx
+
+    def sampler(self, B, guided, shape, cap_shape):
+        """The SamplerGraph of one (batch, CFG or not, latent shape, caption shape) in the current precision and
+        deterministic mode, captured on first use and kept until release_sampler_graphs() or a rebind of the weights."""
+        key = (B, bool(guided), tuple(shape), tuple(cap_shape), self.ops.prec, self.ops._det_ws is not None)
+        g = self._sampler_graphs.get(key)
+        if g is None:
+            g = self._sampler_graphs[key] = SamplerGraph(self, B, guided, shape, cap_shape)
+        return g
+
+    def release_sampler_graphs(self):
+        """Drop every captured sampler graph and the memory pool they hold."""
+        self._sampler_graphs.clear()
+
     def forward_raw(self, x, t, cap, mask_ratio=0.0, mask_noise=None, keep=False):
         """DiT.forward_without_cfg (dit.py:455-519): (F_x, mask).  keep=True saves the activations and returns
         (F_x, mask, ctx) for backward_output(ctx, ...)."""
@@ -829,3 +855,130 @@ class Engine:
     weights_token = None  # callable -> hashable; set by models.dit.DiT
     on_backbone_grads_ready = None  # optional callable, see backward()
     mask_token: Optional[torch.Tensor] = None
+
+
+class SamplerGraph:
+    """The Heun sampler of LatentDiffusion._heun as replays of captured CUDA graphs.
+
+    Three graphs share one memory pool: the prompt cache of the caption (Engine.prompt_cache), one full Heun step
+    (stage in -> denoiser -> euler -> denoiser -> correct -> step + 1) and the last step (stage in -> denoiser -> euler ->
+    step + 1).  Every per-step value lives in device memory -- the schedule table, the step index, the pre-drawn noise,
+    the guidance scale -- so a run is a fixed sequence of replays with no host decision and no host sync in between.
+    Static buffers: the fp64 state x / x_hat / d_cur, the fp32 denoiser input and sigma (doubled for CFG), the caption
+    (with the zero half for CFG), the table, the step index and the noise of `max_steps` steps (grown, with a recapture,
+    when a run asks for more)."""
+
+    def __init__(self, eng, B, guided, shape, cap_shape):
+        dev = eng.ops.device
+        f64 = torch.float64
+        self.eng, self.B, self.guided = eng, B, bool(guided)
+        B2 = 2 * B if guided else B
+        self.x = torch.zeros((B, *shape), dtype=f64, device=dev)
+        self.x_hat = torch.zeros_like(self.x)
+        self.d_cur = torch.zeros_like(self.x)
+        self.xin = torch.zeros((B2, *shape), dtype=F32, device=dev)
+        self.sigma = torch.ones((B2,), dtype=F32, device=dev)
+        self.cap = torch.zeros((B2, *cap_shape), dtype=torch.float16, device=dev)
+        self.cfg = torch.ones((1,), dtype=F32, device=dev)
+        self.step = torch.zeros((1,), dtype=torch.int32, device=dev)
+        self.max_steps = 0
+        self.table = self.noise = None  # device table and noise, sized for max_steps
+        self.graphs = None
+        self.den = {}       # graph name -> the denoiser outputs D of its calls (static addresses in the pool)
+        self.captures = 0   # number of captures so far (a replay of an unchanged setting does not recapture)
+        self.runs = 0       # sampler runs served
+        self.pool = None
+
+    def _stage(self, stage, den=None):
+        o = self.eng.ops
+        o.edm_heun(stage, self.x, self.x_hat, self.d_cur, den, self.noise if stage == o.HEUN_IN else None,
+                   None if stage == o.HEUN_CORRECT else self.xin, self.sigma, self.table, self.step, self.s_noise)
+
+    def _denoise(self):
+        eng, edm = self.eng, self.edm
+        if self.guided:
+            return eng.denoise_cfg(self.xin, self.sigma, self.cfg, edm, self.pc)
+        return eng.denoise(self.xin, self.sigma, None, 0.0, None, edm, prompt=self.pc)[0]
+
+    def _body(self, name):
+        """What one graph holds; the same launches run eagerly for the warm-up."""
+        o = self.eng.ops
+        if name == "prompt":
+            self.pc = self.eng.prompt_cache(self.cap)
+            return
+        self._stage(o.HEUN_IN)
+        dens = [self._denoise()]
+        self._stage(o.HEUN_EULER, dens[0])
+        if name == "step":
+            dens.append(self._denoise())
+            self._stage(o.HEUN_CORRECT, dens[1])
+        o.edm_heun(o.HEUN_NEXT, None, None, None, None, None, None, None, None, self.step, 1.0)
+        self.den[name] = dens
+
+    def _capture(self):
+        # warm-up: every launch once outside capture (tensor-map cache, cudaFuncSetAttribute, lazy module loads), on the
+        # run's own inputs; the caller re-writes the state before replaying
+        for name in ("prompt", "step", "last"):
+            self.step.zero_()
+            self._body(name)
+        self.pool = torch.cuda.graph_pool_handle()
+        self.graphs = {}
+        for name in ("prompt", "step", "last"):
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=self.pool):
+                self._body(name)
+            self.graphs[name] = g
+        self.captures += 1
+
+    def run(self, x0, t_steps, t_hat, noise, cap, cfg, s_noise, edm, debug=None):
+        """x0 f64 [B,C,H,W] = x * t_steps[0]; t_steps / t_hat: host f64 (n+1 / n values); noise: the n draws of the eager
+        loop; cap: fp16 caption [B, ...].  Returns the final state in fp32, like _heun.  `debug(k, call, D)` (optional) sees
+        the denoiser output of every call after the replay that made it."""
+        eng, o = self.eng, self.eng.ops
+        n = len(t_hat)
+        token = eng.weights_token() if eng.weights_token is not None else None
+        eng.store.refresh_copies(o, token)  # weights updated since the capture: new bf16 copies, outside the graphs
+        if n > self.max_steps or s_noise != getattr(self, "s_noise", s_noise) or edm != getattr(self, "edm", edm):
+            self.graphs, self.den, self.pc = None, {}, None
+            if n > self.max_steps:
+                self.max_steps = n
+                self.table = torch.zeros(2 * n + 1, dtype=torch.float64, device=o.device)
+                self.noise = torch.zeros((n, *self.x.shape), dtype=torch.float64, device=o.device)
+        self.s_noise, self.edm = s_noise, dict(edm)
+        self.table.copy_(SamplerGraph.schedule_table(t_steps, t_hat, self.max_steps))
+        for k, nk in enumerate(noise):
+            self.noise[k].copy_(nk)
+        B = self.B
+        self.cap[:B].copy_(cap)
+        if self.guided:
+            self.cap[B:].zero_()
+            self.cfg.fill_(cfg)
+        if self.graphs is None:
+            self.x.copy_(x0)
+            self._capture()
+        self.x.copy_(x0)
+        self.step.zero_()
+        self._replay(n, debug)
+        self.runs += 1
+        return self.x.to(torch.float32)
+
+    def _replay(self, n, debug):
+        """The run itself: graph replays only, nothing that waits for the device."""
+        g = self.graphs
+        g["prompt"].replay()
+        for k in range(n):
+            name = "last" if k == n - 1 else "step"
+            g[name].replay()
+            if debug is not None:
+                for j, d in enumerate(self.den[name]):
+                    debug(k, j, d)
+
+    @staticmethod
+    def schedule_table(t_steps, t_hat, max_steps):
+        """The schedule table md_edm_heun reads (host f64 [2*max_steps+1]): t_steps (n+1 values, the last one 0) at
+        [0, n], t_hat (n values) at [max_steps+1, max_steps+1+n), zeros elsewhere."""
+        n = len(t_hat)
+        tab = torch.zeros(2 * max_steps + 1, dtype=torch.float64)
+        tab[:n + 1] = t_steps
+        tab[max_steps + 1:max_steps + 1 + n] = t_hat
+        return tab

@@ -92,6 +92,10 @@ class LatentDiffusion(_Base):
         self.last_per_sample_loss = None
         self.cache_prompt = True  # sampler fast path: caption-only work once per edm_sampler_loop (engine.prompt_cache)
         self._prompt_memo = None
+        # sampler fast path: the Heun loop as replays of captured CUDA graphs where _sampler_graph_eligible holds; False
+        # keeps the eager loop (A/B runs, and the comparator of the graph path's tests)
+        self.sampler_graph = True
+        self.sampler_debug = None  # optional callable(step, call, D): sees the fp32 denoiser output of every sampler call
 
     def _edm_scalars(self):
         e = self.edm_config
@@ -169,11 +173,7 @@ class LatentDiffusion(_Base):
         when `model_forward_fxn` is this model's own DiT (plain or CFG partial) and no gradient is wanted; under grad
         mode with x, sigma, y or a DiT parameter requiring grad, and for any other function, the reference's own
         composition c_skip*x + c_out*F(c_in*x, ln(sigma)/4, y) runs over the (differentiable) DiT.forward."""
-        fn, cfg = model_forward_fxn, 1.0
-        if isinstance(fn, partial) and getattr(fn.func, "__self__", None) is self.dit:
-            cfg = fn.keywords.get("cfg", 1.0)
-            fn = fn.func
-        own = fn is self.dit or getattr(fn, "__self__", None) is self.dit
+        own, cfg = self._own_forward(model_forward_fxn)
         B = x.shape[0]
         sigma_b = sigma.to(torch.float32).reshape(-1).expand(B).contiguous()
         fused = own and not self._wants_grad(x, sigma, y)
@@ -215,6 +215,15 @@ class LatentDiffusion(_Base):
         out["sample"] = c_skip * x + c_out * out["sample"]
         return out
 
+    def _own_forward(self, fn):
+        """(True, cfg) when fn is this model's own DiT -- the module, its forward, or the CFG partial of its forward --
+        and (False, 1.0) for any other function."""
+        cfg = 1.0
+        if isinstance(fn, partial) and getattr(fn.func, "__self__", None) is self.dit:
+            cfg = fn.keywords.get("cfg", 1.0)
+            fn = fn.func
+        return fn is self.dit or getattr(fn, "__self__", None) is self.dit, cfg
+
     def _wants_grad(self, x, sigma, y) -> bool:
         """Grad mode is on and a gradient is wanted for an input or for the DiT's parameters."""
         if not torch.is_grad_enabled():
@@ -239,23 +248,68 @@ class LatentDiffusion(_Base):
         metric.update(outputs[0])
 
     # ------------------------------------------------------------------ sampler (model.py:231-353)
-    @torch.no_grad()
     def edm_sampler_loop(self, x: torch.Tensor, y: torch.Tensor, steps: Optional[int] = None, cfg: float = 1.0, **kwargs):
-        """Heun sampler with fp64 state (model.py:232-297); every denoiser call goes through the fused kernels."""
-        e = self.edm_config
+        """Heun sampler with fp64 state (model.py:232-297); every denoiser call goes through the fused kernels.  Where
+        _sampler_graph_eligible holds, the whole loop runs as replays of captured CUDA graphs (engine.SamplerGraph),
+        bit-identical to the eager loop and drawing the same random numbers; everywhere else the eager loop runs."""
         fwd = partial(self.dit.forward, cfg=cfg) if cfg > 1.0 else self.dit.forward
-        n = e.num_steps if steps is None else steps
-        i = torch.arange(n, dtype=torch.float64, device=x.device)
-        t_steps = (e.sigma_max ** (1 / e.rho) + i / (n - 1) * (e.sigma_min ** (1 / e.rho) - e.sigma_max ** (1 / e.rho))) ** e.rho
-        t_steps = torch.cat([torch.as_tensor(t_steps), torch.zeros_like(t_steps[:1])])
-        x_next = x.to(torch.float64) * t_steps[0]
-        # the caption is the same tensor for all 2n-1 denoiser calls: its stem and the 34 cross-attention K/V projections
-        # are computed once (engine.prompt_cache) -- the reference recomputes them per call (dit.py:481-485, utils.py:116-129)
-        self._prompt_memo = {"y": y, "cfg": cfg if cfg > 1.0 else 1.0, "pc": None, "cap": None} if self.cache_prompt else None
-        try:
-            return self._heun(x_next, t_steps, y, fwd, n, **kwargs)
-        finally:
-            self._prompt_memo = None
+        graph = self._sampler_graph_eligible(fwd, x, y, kwargs)  # in the caller's grad mode
+        with torch.no_grad():
+            e = self.edm_config
+            n = e.num_steps if steps is None else steps
+            i = torch.arange(n, dtype=torch.float64, device=x.device)
+            t_steps = (e.sigma_max ** (1 / e.rho) + i / (n - 1) * (e.sigma_min ** (1 / e.rho) - e.sigma_max ** (1 / e.rho))) ** e.rho
+            t_steps = torch.cat([torch.as_tensor(t_steps), torch.zeros_like(t_steps[:1])])
+            x_next = x.to(torch.float64) * t_steps[0]
+            if graph:
+                return self._heun_graph(x_next, t_steps, y, cfg if cfg > 1.0 else 1.0, n)
+            # the caption is the same tensor for all 2n-1 denoiser calls: its stem and the 34 cross-attention K/V projections
+            # are computed once (engine.prompt_cache) -- the reference recomputes them per call (dit.py:481-485,
+            # utils.py:116-129)
+            self._prompt_memo = {"y": y, "cfg": cfg if cfg > 1.0 else 1.0, "pc": None, "cap": None} if self.cache_prompt else None
+            try:
+                return self._heun(x_next, t_steps, y, fwd, n, **kwargs)
+            finally:
+                self._prompt_memo = None
+
+    def _sampler_graph_eligible(self, fwd, x, y, kwargs) -> bool:
+        """The rule for the CUDA-graph sampler: the CUDA ops, the model's own DiT as the denoiser with no extra keyword
+        arguments, the prompt cache on, model_forward_wrapper not overridden, no gradient wanted for x or y, and
+        sampler_graph not switched off.  Anything else keeps the eager loop, whose semantics it then defines."""
+        from ..ops import CudaOps
+        if not (self.sampler_graph and self.cache_prompt) or kwargs or not self._own_forward(fwd)[0]:
+            return False
+        if type(self).model_forward_wrapper is not LatentDiffusion.model_forward_wrapper:
+            return False
+        if torch.is_grad_enabled() and any(torch.is_tensor(v) and v.requires_grad for v in (x, y)):
+            return False
+        return isinstance(self.dit.engine.ops, CudaOps)
+
+    def _heun_schedule(self, t_steps, n):
+        """(t_steps, t_hat) on the host in fp64: the values _heun computes per step, the S_churn window's gamma decided
+        with the same expressions, once per run."""
+        e = self.edm_config
+        t_cpu = t_steps.cpu()
+        t_hat = []
+        for t_cur in t_cpu[:n]:
+            gamma = min(e.S_churn / n, np.sqrt(2) - 1) if e.S_min <= t_cur <= e.S_max else 0
+            t_hat.append(torch.as_tensor(t_cur + gamma * t_cur))
+        return t_cpu, torch.stack(t_hat) if t_hat else torch.zeros(0, dtype=torch.float64)
+
+    def _predraw_noise(self, x_cur, n):
+        """The n draws self.randn_like(x_cur) of the eager loop, in its order (the denoiser draws nothing at mask ratio
+        0), so that the values and the generator state afterwards are the eager loop's."""
+        return [self.randn_like(x_cur) for _ in range(n)]
+
+    def _heun_graph(self, x_next, t_steps, y, cfg, n):
+        t_cpu, t_hat = self._heun_schedule(t_steps, n)
+        noise = self._predraw_noise(x_next, n)
+        cap = self.dit._caption_f16(y)
+        B = x_next.shape[0]
+        eng = self.dit.engine
+        sg = eng.sampler(B, cfg != 1.0, tuple(x_next.shape[1:]), tuple(cap.shape[1:]))
+        return sg.run(x_next, t_cpu, t_hat, noise, cap, cfg, self.edm_config.S_noise, self._edm_scalars(),
+                      debug=self.sampler_debug)
 
     def _heun(self, x_next, t_steps, y, fwd, n, **kwargs):
         e = self.edm_config
@@ -265,12 +319,18 @@ class LatentDiffusion(_Base):
             t_hat = torch.as_tensor(t_cur + gamma * t_cur)
             x_hat = x_cur + (t_hat ** 2 - t_cur ** 2).sqrt() * e.S_noise * self.randn_like(x_cur)
             den = self.model_forward_wrapper(x_hat.to(torch.float32), t_hat.to(torch.float32), y, fwd, mask_ratio=0,
-                                             **kwargs)["sample"].to(torch.float64)
+                                             **kwargs)["sample"]
+            if self.sampler_debug is not None:
+                self.sampler_debug(k, 0, den)
+            den = den.to(torch.float64)
             d_cur = (x_hat - den) / t_hat
             x_next = x_hat + (t_next - t_hat) * d_cur
             if k < n - 1:
                 den = self.model_forward_wrapper(x_next.to(torch.float32), t_next.to(torch.float32), y, fwd,
-                                                 mask_ratio=0, **kwargs)["sample"].to(torch.float64)
+                                                 mask_ratio=0, **kwargs)["sample"]
+                if self.sampler_debug is not None:
+                    self.sampler_debug(k, 1, den)
+                den = den.to(torch.float64)
                 d_prime = (x_next - den) / t_next
                 x_next = x_hat + (t_next - t_hat) * (0.5 * d_cur + 0.5 * d_prime)
         return x_next.to(torch.float32)

@@ -24,6 +24,7 @@ _I64 = C.c_int64
 _F = C.c_float
 _P = C.c_void_p
 _I = C.c_int
+_D = C.c_double
 
 _PROTOS = {
     "md_ln_fwd": [_P, _I, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P, _P, _P, _I64, _I64, _F, _I, _P],
@@ -67,6 +68,8 @@ _PROTOS = {
     "md_edm_loss_fwd": [_P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _P],
     "md_edm_loss_bwd": [_P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _I, _P],
     "md_edm_output": [_P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _P],
+    "md_edm_heun": [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _D, _P],
+    "md_edm_output_cfg": [_P, _P, _P, _P, _P, _F, _F, _I64, _I64, _I64, _I64, _I64, _P],
     "md_unpatchify_bwd": [_P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _I, _P],
     "md_patchify_bwd": [_P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I, _P],
     "md_timestep_embed_bwd": [_P, _P, _P, _I64, _I64, _I, _P],
@@ -476,6 +479,45 @@ class CudaOps:
         B, Cc, H, W = ref.shape
         self._call("md_edm_output", ftok.data_ptr(), _ptr(ids_restore), _ptr(mask_token), _ptr(xn), _ptr(coef),
                    _ptr(fx), _ptr(dx), B, Cc, H, W, p, Tk)
+
+    HEUN_IN, HEUN_EULER, HEUN_CORRECT, HEUN_NEXT = 0, 1, 2, 3
+
+    def edm_heun(self, stage, x, x_hat, d_cur, den, noise, xin, sigma, table, step, s_noise):
+        """One stage of the fp64 Heun step (md_edm_heun) on the state x, x_hat, d_cur (f64 [B,C,H,W]).  table: f64
+        [2*max_steps+1] (t_steps | t_hat), step: int32 [1] device index, noise: f64 [max_steps, B,C,H,W], xin: f32 [copies*B,
+        C,H,W], sigma: f32 [copies*B], den: f32 [B,C,H,W].  HEUN_NEXT only advances `step`."""
+        assert step.dtype == torch.int32 and step.numel() == 1
+        if stage == self.HEUN_NEXT:
+            self._call("md_edm_heun", stage, *([None] * 8), step.data_ptr(), 1, 1, 1, 1, 1.0)
+            return
+        B = x.shape[0]
+        n = x[0].numel()
+        assert table.dtype == torch.float64 and table.numel() % 2 == 1 and table.is_contiguous()
+        max_steps = table.numel() // 2
+        for t in (x, x_hat, d_cur):
+            assert t is None or (t.dtype == torch.float64 and t.shape == x.shape and t.is_contiguous())
+        assert den is None or (den.dtype == torch.float32 and den.shape == x.shape and den.is_contiguous())
+        assert noise is None or (noise.dtype == torch.float64 and noise.is_contiguous() and
+                                 tuple(noise.shape) == (max_steps, *x.shape))
+        copies = 1
+        if xin is not None:
+            copies = xin.shape[0] // B
+            assert xin.dtype == torch.float32 and xin.is_contiguous() and tuple(xin.shape) == (copies * B, *x.shape[1:])
+            assert sigma.dtype == torch.float32 and sigma.numel() == copies * B
+        self._call("md_edm_heun", stage, x.data_ptr(), _ptr(x_hat), _ptr(d_cur), _ptr(den), _ptr(noise), _ptr(xin),
+                   _ptr(sigma), table.data_ptr(), step.data_ptr(), max_steps, B, n, copies, float(s_noise))
+
+    def edm_output_cfg(self, ftok, x, sigma, cfg, dx, sigma_data, p):
+        """dx = c_skip*x + c_out*(unc + cfg*(cond - unc)) for a doubled (cond | uncond) batch, md_edm_output_cfg: ftok f32
+        [2B*T, p*p*C], x / dx f32 [B,C,H,W], sigma f32 [B], cfg f32 [1] on the device.  sigma_data is the Python float of
+        the EDM config: its fp32 value and the fp32 value of its square enter like torch's scalar operands."""
+        B, Cc, H, W = dx.shape
+        assert x.shape == dx.shape and x.is_contiguous() and dx.is_contiguous() and x.dtype == dx.dtype == torch.float32
+        assert ftok.dtype == torch.float32 and ftok.is_contiguous() and tuple(ftok.shape) == (2 * B * (H // p) * (W // p),
+                                                                                               p * p * Cc)
+        assert sigma.dtype == torch.float32 and sigma.numel() >= B and cfg.dtype == torch.float32 and cfg.numel() == 1
+        self._call("md_edm_output_cfg", ftok.data_ptr(), x.data_ptr(), sigma.data_ptr(), cfg.data_ptr(), dx.data_ptr(),
+                   float(sigma_data), float(sigma_data) ** 2, B, Cc, H, W, p)
 
     # ------------------------------------------------------------------ adjoints of the DiT input / output maps
     def unpatchify_bwd(self, dF, keep_rows, dftok, p, Tk):
